@@ -52,6 +52,21 @@ def dense_packing_lp_model(n_vars: int, n_cons: int, seed: int = 12345) -> dict:
             "constraints": constraints, "variables": variables}
 
 
+def dense_packing_multi_model(n_vars: int, n_cons: int, n_objectives: int, seed: int = 12345) -> dict:
+    """dense_packing_lp_model with `optimize` = {profit: max, attr1: max, ...}: the extra objective attributes are
+    U{1..50} per variable, drawn from the same seed after the packing instance."""
+    rng = np.random.default_rng(seed)
+    rng.integers(1, 21, size=(n_cons, n_vars)); rng.integers(100, 501, size=n_cons); rng.integers(1, 51, size=n_vars)
+    extra = rng.integers(1, 51, size=(n_objectives - 1, n_vars)).astype(np.float64)
+    m = dense_packing_lp_model(n_vars, n_cons, seed)
+    m["name"] = f"DensePacking{n_objectives}obj_{n_vars}x{n_cons}_seed{seed}"
+    m["optimize"] = {"profit": "max", **{f"attr{k}": "max" for k in range(1, n_objectives)}}
+    for j, v in enumerate(m["variables"].values()):
+        for k in range(1, n_objectives):
+            v[f"attr{k}"] = float(extra[k - 1, j])
+    return m
+
+
 def mixed_lp_model(n_vars: int, n_cons: int, seed: int = 7, density: float = 0.7, frac_min: float = 0.3) -> dict:
     """generateRandomLP-like instance (problem-generator.ts:54-108) with a share of `min` rows so
     that phase 1 has work; rhs of `min` rows is kept small so most instances stay feasible."""

@@ -4,7 +4,9 @@ from __future__ import annotations
 
 from typing import Any, Optional
 
+from . import validation
 from .model import Model, object_keys
+from .polyopt import Polyopt
 
 
 class Solver:
@@ -20,15 +22,24 @@ class Solver:
 
     def Solve(self, model: Any, precision: Optional[float] = None, full: bool = False, validate: bool = False):
         if validate:
-            raise NotImplementedError("validation.ts stays host-side TypeScript; not part of the GPU path")
+            model = validation.validate(model)  # main.ts:101-108
         if not model:
             raise ValueError("Solver requires a model to operate on")  # main.ts:110-112
         if isinstance(model, dict):
             opt = model.get("optimize")
-            if isinstance(opt, dict) and len(opt) > 1:
-                raise NotImplementedError("multi-objective (polyopt.ts) is a caller of Solve; out of scope")
+            if isinstance(opt, dict) and len(opt) > 1:  # main.ts:115-119
+                return Polyopt(self, model)
             if model.get("external"):
                 raise NotImplementedError("external solvers (src/external) are out of scope")
+        instance = self._instance(model, precision)
+        solution = instance.solve()
+        return self._finish(instance, solution, full)
+
+    def MultiObjective(self, model: dict):  # main.ts:209-211
+        return Polyopt(self, model)
+
+    def _instance(self, model: Any, precision: Optional[float]) -> Model:
+        if isinstance(model, dict):
             options = model.get("options") or {}
             instance = Model(precision).loadJson(model)
             # selectBranchAndCutService (main.ts:62-83): incremental if explicitly asked, else enhanced if a strategy is named
@@ -42,7 +53,9 @@ class Solver:
         instance.tableau.node_slots = self.node_slots
         instance.tableau.slot_steps = self.slot_steps
         instance.tableau.options.update(self.options)
-        solution = instance.solve()
+        return instance
+
+    def _finish(self, instance: Model, solution, full: bool):  # main.ts:137-146
         self.lastSolvedModel = instance
         solution.solutionSet = solution.generateSolutionSet()
         if full:
