@@ -285,7 +285,6 @@ extern "C" int jslp_tab_create(jslp_ctx *ctx, int width, int height, int row_cap
     if (rc) { delete t; return rc; }
     CK(cudaMalloc(&t->hd.vcol, sizeof(int) * (size_t)t->stride));  // stride entries: addVariable grows W in place
     CK(cudaMalloc(&t->hd.prow, sizeof(double) * (size_t)t->stride));
-    CK(cudaMalloc(&t->hd.crow, sizeof(double) * (size_t)t->stride));
     CK(cudaMalloc(&t->hd.optflag, (size_t)t->stride));
     t->hd.plog_cap = 4096;
     CK(cudaMalloc(&t->hd.plog, sizeof(int4) * (size_t)t->hd.plog_cap));
@@ -326,7 +325,7 @@ extern "C" void jslp_tab_destroy(jslp_tab *t) {
     cudaFree(t->hd.M); cudaFree(t->hd.vrow); cudaFree(t->hd.vcol); cudaFree(t->hd.unres);
     cudaFree(t->hd.opt); cudaFree(t->hd.prow); cudaFree(t->hd.pcol); cudaFree(t->hd.optcoef);
     cudaFree(t->hd.plog); cudaFree(t->hd.optflag); cudaFree(t->hd.intpos);
-    cudaFree(t->hd.part); cudaFree(t->hd.dbg); cudaFree(t->hd.M2); cudaFree(t->hd.crow);
+    cudaFree(t->hd.part); cudaFree(t->hd.dbg); cudaFree(t->hd.M2);
     cudaFree(t->d_T); cudaFree(t->d_rec); cudaFree(t->d_mip); cudaFree(t->d_cuts);
     cudaFreeHost(t->h_rec); cudaFreeHost(t->h_log); cudaFreeHost(t->h_mip); cudaFreeHost(t->h_cuts);
     cudaFree(t->d_count); cudaFreeHost(t->h_count);

@@ -128,7 +128,6 @@ static int ensure_slots(jslp_tab *t, int B, int need_rowcap) {
         CK(cudaMalloc(&ns.M, sizeof(double) * tab * B));
         CK(cudaMalloc(&ns.M2, sizeof(double) * tab * B));
         CK(cudaMalloc(&ns.prow, sizeof(double) * (size_t)stride * B));
-        CK(cudaMalloc(&ns.crow, sizeof(double) * (size_t)stride * B));
         CK(cudaMalloc(&ns.pcol, sizeof(double) * (size_t)rowcap * B));
         CK(cudaMalloc(&ns.vrow, sizeof(int) * (size_t)rowcap * B));
         CK(cudaMalloc(&ns.vcol, sizeof(int) * (size_t)t->W * B));
@@ -150,7 +149,7 @@ static int ensure_slots(jslp_tab *t, int B, int need_rowcap) {
         for (int b = 0; b < B; b++) {
             TabDev &d = hd[b];
             d.M = ns.M + tab * b; d.M2 = ns.M2 + tab * b;
-            d.prow = ns.prow + (size_t)stride * b; d.crow = ns.crow + (size_t)stride * b;
+            d.prow = ns.prow + (size_t)stride * b;
             d.pcol = ns.pcol + (size_t)rowcap * b;
             d.vrow = ns.vrow + (size_t)rowcap * b; d.vcol = ns.vcol + (size_t)t->W * b;
             d.part = ns.part + (size_t)(ctx->num_sms * 16) * b;

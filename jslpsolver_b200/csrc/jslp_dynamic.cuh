@@ -323,7 +323,7 @@ static int restride(jslp_tab *t, int new_stride) {
     };
     int rc;
     if ((rc = widen2d(&t->hd.M, t->rowcap)) || (rc = widen2d(&t->hd.M2, t->rowcap)) || (rc = widen2d(&t->hd.prow, 1)) ||
-        (rc = widen2d(&t->hd.crow, 1)) || (rc = widen2d(&t->hd.opt, t->nOpt)))
+        (rc = widen2d(&t->hd.opt, t->nOpt)))
         return rc;
     int *vc = nullptr;
     CK(cudaMalloc(&vc, sizeof(int) * (size_t)new_stride));

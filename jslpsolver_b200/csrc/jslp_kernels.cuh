@@ -46,7 +46,6 @@ struct TabDev {
     int *intpos;           // position in model.integerVariables by var index, -1 otherwise [n_index]
     double *M2;            // ping-pong partner of M (same shape): the fused ping-pong step reads M, writes
                            // M2 and swaps the two pointers in this descriptor
-    double *crow;          // scratch: cost row as the pivot being staged will leave it [stride]
     Part *part;            // per-CTA look-ahead ratio-test partials [grid]
     long long *dbg;        // optional per-CTA timeline (8 x int64 per CTA per launch) or nullptr
     int W, H, stride, rowcap;
@@ -83,7 +82,7 @@ struct __align__(128) Rec {
     int unbounded_var;
     int only_phase;  // 0 = simplex(), 1 = phase1() only, 2 = phase2() only
     unsigned int ticket;
-    unsigned int arrive;  // ping-pong step: row CTAs that have published their ratio-test partial
+    int pad0;
     int lookahead;   // host switch: 1 = the tail also prices the pivot after next
     int next_c;      // entering column of the NEXT pivot, priced on the cost row as it will be after
                      // the staged pivot: -1 unknown (generic tail), 0 none (optimal), >0 column
@@ -105,6 +104,12 @@ struct MipOut {
     double value;
 };
 
+// One cut of addCutConstraints (cutting-strategies.ts:36-71): type 0 = "min", 1 = "max".
+struct CutDev {
+    int type, var_index;
+    double value;
+};
+
 __device__ __forceinline__ bool nz16(double v) { return !(v >= -1e-16 && v <= 1e-16); }
 
 // IEEE fp64 division.  Inline in the step kernels (a call costs more than the expansion on their
@@ -120,11 +125,8 @@ __device__ __noinline__ double ddiv_z(double a, double b) {
     return a / b;
 }
 
+// Tableau loads bypass L1: other CTAs may just have rewritten the entry in L2.
 __device__ __forceinline__ double ldg_cg(const double *p) { return __ldcg(p); }
-// GLOBAL = tableau lives in HBM/L2 and may just have been rewritten by other CTAs (bypass L1);
-// !GLOBAL = tableau lives in this CTA's shared memory (generic pointers, plain loads).
-template <bool GLOBAL>
-__device__ __forceinline__ double ldt(const double *p) { return GLOBAL ? __ldcg(p) : *p; }
 
 // JS Math.round: nearest, ties toward +inf
 __device__ __forceinline__ double js_round(double x) {
@@ -142,6 +144,112 @@ template <bool IS_MIN>
 __device__ __forceinline__ bool better(const VI &b, const VI &a) {
     if (IS_MIN) return b.v < a.v || (b.v == a.v && b.i < a.i);
     return b.v > a.v || (b.v == a.v && b.i < a.i);
+}
+
+// ---- element rules of the simplex (simplex.ts), each written once for every kernel ---------------------------
+// Values in, values out: the callers issue every load of a pass first and then apply these, so a selector pass stays
+// one L2 round trip.  DIV = the fp64 division: the inline ddiv in the step kernels, ddiv_z in k_node_batch.
+using DivFn = double (*)(double, double);
+
+// Normalised pivot-row entry from its raw value v (simplex.ts:352-364): v / q where |v| > 1e-16, 1 / q in the pivot
+// column, 0 elsewhere.  With `flush` (a row other than the pivot row is updated, simplex.ts:380-382) a quotient that is
+// itself within 1e-16 of zero is stored as 0.
+template <DivFn DIV = ddiv>
+__device__ __forceinline__ double norm_entry(double v, bool is_pc, double q, bool flush) {
+    double f = (is_pc || nz16(v)) ? DIV(is_pc ? 1.0 : v, q) : 0.0;
+    if (flush && !nz16(f) && f != 0.0) f = 0.0;
+    return f;
+}
+
+// Entry of a row with a non-zero pivot-column entry coef after the pivot (simplex.ts:376-386): -coef / q in the pivot
+// column, old - coef * f (two roundings) where the normalised pivot-row entry f is non-zero, old elsewhere.
+template <DivFn DIV = ddiv>
+__device__ __forceinline__ double upd_entry(double old, double coef, double f, bool is_pc, double q) {
+    if (is_pc) return DIV(-coef, q);
+    return nz16(f) ? __dsub_rn(old, __dmul_rn(coef, f)) : old;
+}
+
+// Entry (r, c) of the tableau as the pivot (rstar, cstar, q) leaves it, from its old value (simplex.ts:352-391):
+// is_prow = r is the pivot row, coef = the row's old pivot-column entry, f = the normalised pivot-row entry of column c.
+// A row with |coef| <= 1e-16 is untouched, its pivot-column entry included (:389-391 repeats :371's test: dead code).
+template <DivFn DIV = ddiv>
+__device__ __forceinline__ double new_entry(double old, bool is_prow, double coef, double f, bool is_pc, double q) {
+    if (is_prow) return f;
+    return nz16(coef) ? upd_entry<DIV>(old, coef, f, is_pc, q) : old;
+}
+
+// Cost-row entry after the staged pivot (cstar, q) from the RAW pivot-row entry v: new_entry on norm_entry(v), and v
+// is divided only where the cost row changes (coef0 = the cost row's pivot-column entry).  The flush is left out: an f
+// within 1e-16 of zero leaves the entry alone either way.
+template <DivFn DIV = ddiv>
+__device__ __forceinline__ double priced_cost(double cost, double v, double coef0, bool is_pc, double q) {
+    const double f = (nz16(coef0) && !is_pc) ? norm_entry<DIV>(v, false, q, false) : 0.0;
+    return new_entry<DIV>(cost, false, coef0, f, is_pc, q);
+}
+
+// Lazy-flush flag of a pivot (simplex.ts:380): cnt = rows with a non-zero pivot-column entry, the pivot row included.
+__device__ __forceinline__ bool flush_flag(int cnt, double q) { return cnt - (nz16(q) ? 1 : 0) > 0; }
+
+// One row of the ratio test (simplex.ts:271-296); col / rhs = the row's entries in the entering column and column 0.
+// Rows with |col| >= prec take part: a degenerate one (col > 0, |rhs| < prec) lowers dmin, and the lowest such row
+// wins outright, as the reference's early exit does; any other offers its quotient to best (lowest row on ties when
+// rows come in increasing order).  cnt counts the non-zero entries of the column, row 0 included (flush_flag).
+template <DivFn DIV = ddiv>
+__device__ __forceinline__ void ratio_step(int r, double col, double rhs, bool is_neg, double prec, int &dmin, VI &best,
+                                           int &cnt) {
+    if (nz16(col)) cnt++;
+    if (r == 0 || (-prec < col && col < prec)) return;
+    if (col > 0 && prec > rhs && rhs > -prec) { dmin = min(dmin, r); return; }
+    const double quo = DIV(is_neg ? -rhs : rhs, col);  // (-rhs) / col == -rhs / col
+    if (quo > prec && best.v > quo) { best.v = quo; best.i = r; }
+}
+
+// One column of the phase-1 entering-column scan (simplex.ts:56-76): the column qualifies when its variable is
+// unrestricted or coef (the leaving row's entry) < -prec, and the largest -cost / coef wins (lowest column on ties when
+// columns come in increasing order).  cost() yields the cost-row entry; it runs for qualifying columns only.
+template <DivFn DIV = ddiv, class Cost>
+__device__ __forceinline__ void entering_step(int c, double coef, bool unres, double prec, VI &e, Cost cost) {
+    if (unres || coef < -prec) {
+        const double quo = DIV(-cost(), coef);
+        if (e.v < quo) { e.v = quo; e.i = c; }
+    }
+}
+
+// Pivot (r, c) on thread 0 (simplex.ts:339-349): pivot-log entry and label swap; the inverse maps are rebuilt on
+// read-back.  leaving / entering = the labels of row r and column c before the swap.
+__device__ __forceinline__ void log_pivot(int4 *plog, int log_n, int cap, int *vrow, int *vcol, int phase, int r, int c,
+                                          int leaving, int entering) {
+    if (log_n < cap) plog[log_n] = make_int4(r | (phase == 2 ? (1 << 30) : 0), c, leaving, entering);
+    vrow[r] = entering;
+    vcol[c] = leaving;
+}
+
+// Stages pivot (r, c) on thread 0: log_pivot plus the record fields every staging site writes.
+__device__ __forceinline__ void stage_pivot(const TabDev &T, Rec *rec, int log_n, int phase, int r, int c, int leaving,
+                                            int entering, double q, int isneg, bool flush, int next_c, int prow_norm) {
+    log_pivot(T.plog, log_n, T.plog_cap, T.vrow, T.vcol, phase, r, c, leaving, entering);
+    rec->log_n = log_n + 1;
+    rec->phase = phase; rec->r = r; rec->c = c; rec->q = q; rec->is_neg = isneg; rec->flush = flush;
+    rec->has_pivot = 1;
+    rec->next_c = next_c;        // -1: the pivot after this one has not been priced
+    rec->prow_norm = prow_norm;  // 1: the prow side buffer holds the row already normalised
+}
+
+// Cut rows (addCutConstraints, cutting-strategies.ts:36-71).  cut_lookup: the row where the cut's variable is basic
+// (rows 1 .. H0-1) and its column, -1 where absent, searched from position 1 + first in steps of `step`; the caller
+// merges the threads' answers (a label occurs once).
+__device__ __forceinline__ void cut_lookup(const int *vrow, int H0, const int *vcol, int W, int var, int first, int step,
+                                           int &row, int &col) {
+    row = col = -1;
+    for (int r = 1 + first; r < H0; r += step) if (vrow[r] == var) row = r;
+    for (int c = 1 + first; c < W; c += step) if (vcol[c] == var) col = c;
+}
+// Entry c of the cut row; vr = the row where the variable is basic, nullptr when it is non-basic (in column col, -1
+// when basic) or when c lies in the row padding past W (the entry is then 0).
+__device__ __forceinline__ double cut_entry(const CutDev &cut, int c, int col, const double *vr) {
+    const double sign = cut.type == 0 ? -1.0 : 1.0;
+    if (vr == nullptr) return c == 0 ? sign * cut.value : (c == col ? sign : 0.0);
+    return c == 0 ? sign * (cut.value - vr[0]) : -sign * vr[c];
 }
 
 struct RedSmem {
@@ -297,7 +405,6 @@ __device__ __forceinline__ void block_reduce_ratio(int &dmin, VI &m, int &cnt, R
 // Copies the raw row `src` (W entries) into the stride-long side buffer `dst` (zero padded) with
 // all loads of a pass issued before its stores: the two may alias as far as the compiler knows,
 // and a load/store/load chain would cost one L2 round trip per element.
-template <bool GLOBAL>
 __device__ __forceinline__ void cta_copy_row(double *dst, const double *src, int W, int stride) {
     const int tid = threadIdx.x, NT = blockDim.x;
     for (int c0 = 0; c0 < stride; c0 += 8 * NT) {
@@ -305,7 +412,7 @@ __device__ __forceinline__ void cta_copy_row(double *dst, const double *src, int
 #pragma unroll
         for (int k = 0; k < 8; k++) {
             const int c = c0 + tid + k * NT;
-            v[k] = c < W ? ldt<GLOBAL>(src + c) : 0.0;
+            v[k] = c < W ? ldg_cg(src + c) : 0.0;
         }
 #pragma unroll
         for (int k = 0; k < 8; k++) {
@@ -313,17 +420,6 @@ __device__ __forceinline__ void cta_copy_row(double *dst, const double *src, int
             if (c < stride) dst[c] = v[k];
         }
     }
-}
-
-// Updated cost entry of column c once the pivot (cstar, q) with cost-row coefficient coef0 has been
-// applied: the single-element form of update_rows for row 0.  v = raw pivot-row entry.
-__device__ __forceinline__ double priced_cost(double cost, double v, double coef0, bool nzc, bool is_pc, double q) {
-    if (nzc) {
-        if (is_pc) return ddiv(-coef0, q);
-        const double f = nz16(v) ? ddiv(v, q) : 0.0;
-        return nz16(f) ? __dsub_rn(cost, __dmul_rn(coef0, f)) : cost;
-    }
-    return cost;  // |coef0| <= 1e-16: the cost row is untouched (simplex.ts:371; :389-391 is dead code)
 }
 
 struct SelSmem {
@@ -406,12 +502,11 @@ __device__ __forceinline__ void price_finish_rx(const TabDev &T, SelSmem &s, con
     __syncthreads();
 }
 
-template <bool GLOBAL, bool PRICED>
+template <bool PRICED>
 __device__ __noinline__ void cta_price_scan(const TabDev &T, SelSmem &s, const double *costsrc, const double *rowsrc, double q,
                                double coef0, int cstar, int new_label, int *found_out, int *neg_out) {
     const int tid = threadIdx.x, NT = blockDim.x;
     const int W = T.W;
-    const bool nzc = nz16(coef0);
     const int bsz = T.use_partial ? T.batch_size : max(1, W - 1);
     const bool has_unres = T.unres != nullptr;
     PriceAcc acc;
@@ -422,15 +517,15 @@ __device__ __noinline__ void cta_price_scan(const TabDev &T, SelSmem &s, const d
 #pragma unroll
         for (int k = 0; k < 8; k++) {
             const int c = c0 + tid + k * NT;
-            cv[k] = c < W ? ldt<GLOBAL>(costsrc + c) : 0.0;
-            rv[k] = (PRICED && c < W) ? ldt<GLOBAL>(rowsrc + c) : 0.0;
+            cv[k] = c < W ? ldg_cg(costsrc + c) : 0.0;
+            rv[k] = (PRICED && c < W) ? ldg_cg(rowsrc + c) : 0.0;
         }
 #pragma unroll
         for (int k = 0; k < 8; k++) {
             const int c = c0 + tid + k * NT;
             if (c >= W) continue;
             double nc = cv[k];
-            if (PRICED) nc = priced_cost(nc, rv[k], coef0, nzc, c == cstar, q);
+            if (PRICED) nc = priced_cost(nc, rv[k], coef0, c == cstar, q);
             int label = -1;
             if (has_unres && nc < 0) label = (PRICED && c == cstar) ? new_label : T.vcol[c];
             price_consider(T, acc, c, nc, label, bsz);
@@ -502,40 +597,24 @@ __device__ __noinline__ void price_with_optional_seq(const TabDev &T, int *outCo
 // Stage pivot (rstar, cstar): raw pivot row -> prow, optional pivot-column entries, label swap,
 // pivot log, record.  `cnt` = number of rows r (incl. row 0 and rstar) with a non-zero
 // pivot-column entry; pcol must already be staged.
-template <bool GLOBAL>
 __device__ void cta_stage_pivot(const TabDev &T, Rec *rec, int phase, int rstar, int cstar,
                                 int isneg, int cnt) {
     const int tid = threadIdx.x, NT = blockDim.x;
     const double *prowsrc = T.M + (size_t)rstar * T.stride;
-    const double q = ldt<GLOBAL>(prowsrc + cstar);
+    const double q = ldg_cg(prowsrc + cstar);
     int leaving = 0, entering = 0;
     if (tid == 0) {  // only the thread that swaps the labels may read them (no barrier in between)
         leaving = T.vrow[rstar];
         entering = T.vcol[cstar];
     }
-    cta_copy_row<GLOBAL>(T.prow, prowsrc, T.W, T.stride);
-    for (int o = tid; o < T.nOpt; o += NT) T.optcoef[o] = ldt<GLOBAL>(T.opt + (size_t)o * T.stride + cstar);
-    if (tid == 0) {
-        if (rec->log_n < T.plog_cap) T.plog[rec->log_n] = make_int4(rstar | (phase == 2 ? (1 << 30) : 0), cstar, leaving, entering);
-        rec->log_n += 1;
-        T.vrow[rstar] = entering;  // simplex.ts:339-349 (the inverse maps are rebuilt on read-back)
-        T.vcol[cstar] = leaving;
-        rec->phase = phase;
-        rec->r = rstar;
-        rec->c = cstar;
-        rec->q = q;
-        rec->is_neg = isneg;
-        rec->flush = (cnt - (nz16(q) ? 1 : 0)) > 0;
-        rec->has_pivot = 1;
-        rec->next_c = -1;  // the pivot after this one has not been priced
-        rec->prow_norm = 0;
-    }
+    cta_copy_row(T.prow, prowsrc, T.W, T.stride);
+    for (int o = tid; o < T.nOpt; o += NT) T.optcoef[o] = ldg_cg(T.opt + (size_t)o * T.stride + cstar);
+    if (tid == 0) stage_pivot(T, rec, rec->log_n, phase, rstar, cstar, leaving, entering, q, isneg, flush_flag(cnt, q), -1, 0);
 }
 
 // One CTA decides the next pivot from the tableau as it stands in L2/HBM (phase1: simplex.ts:
 // 38-76, phase2: 129-303) and stages it.  All tableau reads bypass L1 (__ldcg): in the fused
 // kernel this runs after other CTAs have just rewritten the tableau.
-template <bool GLOBAL>
 __device__ __noinline__ void cta_select(const TabDev &T, Rec *rec, SelSmem &s) {
     const int tid = threadIdx.x, NT = blockDim.x;
     const int W = T.W, H = T.H;
@@ -555,7 +634,7 @@ __device__ __noinline__ void cta_select(const TabDev &T, Rec *rec, SelSmem &s) {
 #pragma unroll
             for (int k = 0; k < 8; k++) {
                 const int r = rbase + tid + k * NT;
-                rv[k] = r < H ? ldt<GLOBAL>(M + r * stride) : 0.0;
+                rv[k] = r < H ? ldg_cg(M + r * stride) : 0.0;
             }
 #pragma unroll
             for (int k = 0; k < 8; k++) {
@@ -566,7 +645,7 @@ __device__ __noinline__ void cta_select(const TabDev &T, Rec *rec, SelSmem &s) {
         b = block_reduce_vi<true>(b, init, s.red);
         if (b.i == INT_MAX) {  // feasible (simplex.ts:51-54)
             if (only_phase == 1) {
-                if (tid == 0) { rec->status = ST_P1_DONE; rec->has_pivot = 0; rec->eval_raw = ldt<GLOBAL>(M); }
+                if (tid == 0) { rec->status = ST_P1_DONE; rec->has_pivot = 0; rec->eval_raw = ldg_cg(M); }
                 return;
             }
             phase = 2;
@@ -581,23 +660,18 @@ __device__ __noinline__ void cta_select(const TabDev &T, Rec *rec, SelSmem &s) {
 #pragma unroll
                 for (int k = 0; k < 8; k++) {
                     const int c = c0 + tid + k * NT;
-                    kv[k] = c < W ? ldt<GLOBAL>(lrow + c) : 0.0;
-                    cv[k] = c < W ? ldt<GLOBAL>(M + c) : 0.0;
+                    kv[k] = c < W ? ldg_cg(lrow + c) : 0.0;
+                    cv[k] = c < W ? ldg_cg(M + c) : 0.0;
                 }
 #pragma unroll
                 for (int k = 0; k < 8; k++) {
                     const int c = c0 + tid + k * NT;
-                    if (c >= W) continue;
-                    const double coef = kv[k];
-                    if ((has_unres && is_unres(T, T.vcol[c])) || coef < -prec) {
-                        const double quo = ddiv(-cv[k], coef);
-                        if (e.v < quo) { e.v = quo; e.i = c; }
-                    }
+                    if (c < W) entering_step(c, kv[k], has_unres && is_unres(T, T.vcol[c]), prec, e, [&] { return cv[k]; });
                 }
             }
             e = block_reduce_vi<false>(e, einit, s.red);
             if (e.i == INT_MAX) {  // simplex.ts:73-76
-                if (tid == 0) { rec->status = ST_INFEASIBLE; rec->has_pivot = 0; rec->eval_raw = ldt<GLOBAL>(M); }
+                if (tid == 0) { rec->status = ST_INFEASIBLE; rec->has_pivot = 0; rec->eval_raw = ldg_cg(M); }
                 return;
             }
             cstar = e.i;
@@ -607,7 +681,7 @@ __device__ __noinline__ void cta_select(const TabDev &T, Rec *rec, SelSmem &s) {
     if (rstar < 0) {  // phase 2
         if (T.nOpt == 0) {
             int found, neg;
-            cta_price_scan<GLOBAL, false>(T, s, T.M, nullptr, 1.0, 0.0, -1, -1, &found, &neg);
+            cta_price_scan<false>(T, s, T.M, nullptr, 1.0, 0.0, -1, -1, &found, &neg);
             if (found > 0) { cstar = found; isneg = neg; }
         } else {
             if (tid == 0) {
@@ -622,7 +696,7 @@ __device__ __noinline__ void cta_select(const TabDev &T, Rec *rec, SelSmem &s) {
             __syncthreads();
         }
         if (cstar < 0) {  // optimal (simplex.ts:265-269); setEvaluation rounding is done on the host
-            if (tid == 0) { rec->status = ST_OPTIMAL; rec->phase = 2; rec->has_pivot = 0; rec->eval_raw = ldt<GLOBAL>(M); }
+            if (tid == 0) { rec->status = ST_OPTIMAL; rec->phase = 2; rec->has_pivot = 0; rec->eval_raw = ldg_cg(M); }
             return;
         }
         // ratio test (simplex.ts:271-296) fused with staging of the pivot column
@@ -634,21 +708,15 @@ __device__ __noinline__ void cta_select(const TabDev &T, Rec *rec, SelSmem &s) {
 #pragma unroll
             for (int k = 0; k < 8; k++) {
                 const int r = rbase + tid + k * NT;
-                cv[k] = r < H ? ldt<GLOBAL>(M + r * stride + cstar) : 0.0;
-                rv[k] = r < H ? ldt<GLOBAL>(M + r * stride) : 0.0;
+                cv[k] = r < H ? ldg_cg(M + r * stride + cstar) : 0.0;
+                rv[k] = r < H ? ldg_cg(M + r * stride) : 0.0;
             }
 #pragma unroll
             for (int k = 0; k < 8; k++) {
                 const int r = rbase + tid + k * NT;
                 if (r >= H) continue;
-                const double col = cv[k], rhs = rv[k];
-                T.pcol[r] = col;
-                if (nz16(col)) cnt++;
-                if (r == 0) continue;
-                if (-prec < col && col < prec) continue;
-                if (col > 0 && prec > rhs && rhs > -prec) { dmin = min(dmin, r); continue; }
-                const double quo = ddiv(isneg ? -rhs : rhs, col);
-                if (quo > prec && m.v > quo) { m.v = quo; m.i = r; }
+                T.pcol[r] = cv[k];
+                ratio_step(r, cv[k], rv[k], isneg, prec, dmin, m, cnt);
             }
         }
         block_reduce_ratio(dmin, m, cnt, s.red);
@@ -659,7 +727,7 @@ __device__ __noinline__ void cta_select(const TabDev &T, Rec *rec, SelSmem &s) {
             if (tid == 0) {
                 rec->status = ST_UNBOUNDED; rec->phase = 2; rec->has_pivot = 0;
                 rec->unbounded_var = T.vcol[cstar];
-                rec->eval_raw = ldt<GLOBAL>(M);
+                rec->eval_raw = ldg_cg(M);
             }
             return;
         }
@@ -672,7 +740,7 @@ __device__ __noinline__ void cta_select(const TabDev &T, Rec *rec, SelSmem &s) {
 #pragma unroll
             for (int k = 0; k < 8; k++) {
                 const int r = rbase + tid + k * NT;
-                cv[k] = r < H ? ldt<GLOBAL>(M + r * stride + cstar) : 0.0;
+                cv[k] = r < H ? ldg_cg(M + r * stride + cstar) : 0.0;
             }
 #pragma unroll
             for (int k = 0; k < 8; k++) {
@@ -682,7 +750,7 @@ __device__ __noinline__ void cta_select(const TabDev &T, Rec *rec, SelSmem &s) {
         }
         cnt = block_reduce_int<1>(cnt, s.red);
     }
-    cta_stage_pivot<GLOBAL>(T, rec, phase, rstar, cstar, isneg, cnt);
+    cta_stage_pivot(T, rec, phase, rstar, cstar, isneg, cnt);
 }
 
 __device__ __noinline__ void cta_price_next(const TabDev &T, Rec *rec, SelSmem &s);
@@ -704,12 +772,12 @@ __global__ void __launch_bounds__(512) k_select(const TabDev *Tp, Rec *rec, int 
             if (nz16(col)) cnt++;
         }
         cnt = block_reduce_int<1>(cnt, s.red);
-        cta_stage_pivot<true>(T, rec, rec->phase, force_r, force_c, 0, cnt);
+        cta_stage_pivot(T, rec, rec->phase, force_r, force_c, 0, cnt);
         return;
     }
     if (rec->status != ST_RUNNING || rec->has_pivot) return;
     if (rec->stop_at >= 0 && rec->done >= rec->stop_at) return;
-    cta_select<true>(T, rec, s);
+    cta_select(T, rec, s);
     __syncthreads();
     if (rec->lookahead && rec->has_pivot && rec->phase == 2 && T.nOpt == 0) cta_price_next(T, rec, s);
 }
@@ -775,10 +843,6 @@ __global__ void k_batch_begin(Rec *rec) {
 
 // addCutConstraints (cutting-strategies.ts:36-71): one CTA per cut row, expressed in the
 // current basis.  Cut h becomes row H0 + h with slack index first_index + h.
-struct CutDev {
-    int type, var_index;
-    double value;
-};
 __global__ void __launch_bounds__(256) k_add_cuts(const TabDev *Tp, const CutDev *cuts, int H0, int first_index) {
     __shared__ int s_row, s_col;
     const TabDev &T = *Tp;
@@ -786,27 +850,14 @@ __global__ void __launch_bounds__(256) k_add_cuts(const TabDev *Tp, const CutDev
     const CutDev cut = cuts[h];
     if (tid == 0) { s_row = -1; s_col = -1; }
     __syncthreads();
-    for (int r = 1 + tid; r < H0; r += NT) if (T.vrow[r] == cut.var_index) s_row = r;
-    for (int c = 1 + tid; c < T.W; c += NT) if (T.vcol[c] == cut.var_index) s_col = c;
+    int row, col;
+    cut_lookup(T.vrow, H0, T.vcol, T.W, cut.var_index, tid, NT, row, col);
+    if (row >= 0) s_row = row;
+    if (col >= 0) s_col = col;
     __syncthreads();
-    const double sign = cut.type == 0 ? -1.0 : 1.0;
-    double *crow = T.M + (size_t)(H0 + h) * T.stride;
-    if (s_row < 0) {
-        for (int c = tid; c < T.stride; c += NT) {
-            double v = 0.0;
-            if (c == 0) v = sign * cut.value;
-            else if (c == s_col) v = sign;
-            crow[c] = v;
-        }
-    } else {
-        const double *vr = T.M + (size_t)s_row * T.stride;
-        for (int c = tid; c < T.stride; c += NT) {
-            double v = 0.0;
-            if (c == 0) v = sign * (cut.value - vr[0]);
-            else if (c < T.W) v = -sign * vr[c];
-            crow[c] = v;
-        }
-    }
+    const double *vr = s_row < 0 ? nullptr : T.M + (size_t)s_row * T.stride;
+    double *cutrow = T.M + (size_t)(H0 + h) * T.stride;
+    for (int c = tid; c < T.stride; c += NT) cutrow[c] = cut_entry(cut, c, s_col, c < T.W ? vr : nullptr);
     if (tid == 0) T.vrow[H0 + h] = first_index + h;
 }
 
@@ -931,14 +982,6 @@ __global__ void __launch_bounds__(256) k_mip_scan(const TabDev *Tp, MipOut *out)
     cta_mip_scan(T, out, red);
 }
 
-// Layout conversion between the reference's stride == width matrix and the padded device rows.
-__global__ void k_pack_rows(double *dst, int dstride, const double *src, int sstride, int rows, int cols,
-                            int zero_pad) {
-    const int r = blockIdx.y;
-    if (r >= rows) return;
-    for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < (zero_pad ? dstride : cols); c += gridDim.x * blockDim.x)
-        dst[(size_t)r * dstride + c] = c < cols ? src[(size_t)r * sstride + c] : 0.0;
-}
 // Snapshot / restore of the CURRENT tableau buffer.  The ping-pong step swaps TabDev.M / M2 on the
 // device, so a host-side memcpy enqueued ahead of time cannot know which buffer will be current.
 __global__ void __launch_bounds__(256) k_copy_current(const TabDev *Tp, double *buf, int to_buf) {
@@ -949,11 +992,6 @@ __global__ void __launch_bounds__(256) k_copy_current(const TabDev *Tp, double *
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n2; i += (size_t)gridDim.x * blockDim.x) {
         if (to_buf) b[i] = m[i]; else m[i] = b[i];
     }
-}
-
-__global__ void k_gather_col(double *dst, const double *M, int stride, int rows, int col) {
-    for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < rows; r += gridDim.x * blockDim.x)
-        dst[r] = M[(size_t)r * stride + col];
 }
 
 }  // namespace jslp

@@ -169,19 +169,16 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
     // one warp per cut, no CTA barrier inside
     for (int h = warp; h < nc; h += NW) {
         const CutDev cut = cutS[h];
-        int s_row = -1, s_col = -1;
-        for (int r = 1 + lane; r < H0; r += 32) if (vrow[r] == cut.var_index) s_row = r;
-        for (int c = 1 + lane; c < W; c += 32) if (vcol[c] == cut.var_index) s_col = c;
+        int s_row, s_col;
+        cut_lookup(vrow, H0, vcol, W, cut.var_index, lane, 32, s_row, s_col);
         s_row = __reduce_max_sync(0xffffffffu, s_row);
         s_col = __reduce_max_sync(0xffffffffu, s_col);
-        const double sign = cut.type == 0 ? -1.0 : 1.0;
-        double *crow = Ms + (size_t)(H0 + h) * Ws;
-        if (s_row < 0) {
-            for (int c = lane; c < W; c += 32) crow[c] = c == 0 ? sign * cut.value : (c == s_col ? sign : 0.0);
-        } else {
-            const double *vr = Ms + (size_t)s_row * Ws;
-            for (int c = lane; c < W; c += 32) crow[c] = c == 0 ? sign * (cut.value - vr[0]) : -sign * vr[c];
-        }
+        const double *vr = s_row < 0 ? nullptr : Ms + (size_t)s_row * Ws;
+        double *cutrow = Ms + (size_t)(H0 + h) * Ws;
+        if (vr != nullptr)  // one loop per case: neither tests the case per entry
+            for (int c = lane; c < W; c += 32) cutrow[c] = cut_entry(cut, c, s_col, vr);
+        else
+            for (int c = lane; c < W; c += 32) cutrow[c] = cut_entry(cut, c, s_col, nullptr);
         if (lane == 0) vrow[H0 + h] = nb.first_index + h;
     }
     __syncthreads();
@@ -248,13 +245,8 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
             const double *lrow = Ms + (size_t)slot[sc.r] * Ws;
             VI e = {-INFINITY, INT_MAX};
 #pragma unroll 1
-            for (int c = 1 + tid; c < W; c += NT) {
-                const double coef = lrow[c];
-                if ((has_unres && is_unres(T, vcol[c])) || coef < -prec) {
-                    const double quo = ddiv_z(-cost[c], coef);
-                    if (e.v < quo) { e.v = quo; e.i = c; }
-                }
-            }
+            for (int c = 1 + tid; c < W; c += NT)
+                entering_step<ddiv_z>(c, lrow[c], has_unres && is_unres(T, vcol[c]), prec, e, [&] { return cost[c]; });
             e = warp_reduce_vi<false>(e);
             if (lane == 0) { part.v[warp] = e.v; part.i[warp] = e.i; }
         } else {          // ratio test (simplex.ts:271-296)
@@ -264,13 +256,7 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
 #pragma unroll 1
             for (int r = tid; r < Hn; r += NT) {
                 const double *row = Ms + (size_t)slot[r] * Ws;
-                const double col = row[cs], rv = row[0];
-                if (nz16(col)) cnt++;
-                if (r == 0) continue;
-                if (-prec < col && col < prec) continue;
-                if (col > 0 && prec > rv && rv > -prec) { dmin = min(dmin, r); continue; }
-                const double quo = ddiv_z(neg ? -rv : rv, col);  // (-rhs) / col == -rhs / col
-                if (quo > prec && m.v > quo) { m.v = quo; m.i = r; }
+                ratio_step<ddiv_z>(r, row[cs], row[0], neg, prec, dmin, m, cnt);
             }
             dmin = __reduce_min_sync(0xffffffffu, dmin);
             cnt = __reduce_add_sync(0xffffffffu, cnt);
@@ -309,13 +295,10 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
             }
             if (go) {
                 const double q = Ms[(size_t)slot[rstar] * Ws + cstar];
-                if (lane == 0) {
-                    const int leaving = vrow[rstar], entering = vcol[cstar];
-                    plog[log_n] = make_int4(rstar | (phase == 2 ? (1 << 30) : 0), cstar, leaving, entering);
-                    vrow[rstar] = entering;  // simplex.ts:339-349
-                    vcol[cstar] = leaving;
+                if (lane == 0) {  // log_n < log_cap: checked in S1
+                    log_pivot(plog, log_n, nb.log_cap, vrow, vcol, phase, rstar, cstar, vrow[rstar], vcol[cstar]);
                     piv.go = 1; piv.r = rstar; piv.c = cstar; piv.q = q;
-                    piv.flush = (cnt - (nz16(q) ? 1 : 0)) > 0;
+                    piv.flush = flush_flag(cnt, q);
                 }
                 log_n++;
                 if (phase == 1) p1++; else p2++;
@@ -337,12 +320,7 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
         if (tid < NT / 2) {
             const double *praw = Ms + (size_t)slot[prs] * Ws;
 #pragma unroll 1
-            for (int c = tid; c < W; c += NT / 2) {
-                const double v = praw[c];
-                double f = (c == pcs || nz16(v)) ? ddiv_z(c == pcs ? 1.0 : v, q) : 0.0;
-                if (flush && !nz16(f) && f != 0.0) f = 0.0;
-                frow[c] = f;
-            }
+            for (int c = tid; c < W; c += NT / 2) frow[c] = norm_entry<ddiv_z>(praw[c], c == pcs, q, flush);
         } else {
 #pragma unroll 1
             for (int r = tid - NT / 2; r < Hn; r += NT / 2) {

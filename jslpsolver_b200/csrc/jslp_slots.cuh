@@ -76,27 +76,14 @@ __global__ void __launch_bounds__(256) k_slot_begin(const __grid_constant__ Slot
         __syncthreads();
         if (tid == 0) { s_row = -1; s_col = -1; }
         __syncthreads();
-        for (int r = 1 + tid; r < H0; r += NT) if (sb.root_vrow[r] == cut.var_index) s_row = r;
-        for (int c = 1 + tid; c < T.W; c += NT) if (sb.root_vcol[c] == cut.var_index) s_col = c;
+        int row, col;
+        cut_lookup(sb.root_vrow, H0, sb.root_vcol, T.W, cut.var_index, tid, NT, row, col);
+        if (row >= 0) s_row = row;
+        if (col >= 0) s_col = col;
         __syncthreads();
-        const double sign = cut.type == 0 ? -1.0 : 1.0;
-        double *crow = T.M + (size_t)(H0 + h) * stride;
-        if (s_row < 0) {
-            for (int c = tid; c < stride; c += NT) {
-                double v = 0.0;
-                if (c == 0) v = sign * cut.value;
-                else if (c == s_col) v = sign;
-                crow[c] = v;
-            }
-        } else {
-            const double *vr = sb.rootM + (size_t)s_row * stride;
-            for (int c = tid; c < stride; c += NT) {
-                double v = 0.0;
-                if (c == 0) v = sign * (cut.value - vr[0]);
-                else if (c < T.W) v = -sign * vr[c];
-                crow[c] = v;
-            }
-        }
+        const double *vr = s_row < 0 ? nullptr : sb.rootM + (size_t)s_row * stride;
+        double *cutrow = T.M + (size_t)(H0 + h) * stride;
+        for (int c = tid; c < stride; c += NT) cutrow[c] = cut_entry(cut, c, s_col, c < T.W ? vr : nullptr);
         if (tid == 0) T.vrow[H0 + h] = sb.first_index + h;
     }
     if (blockIdx.x == 0 && tid == 0) {
@@ -137,7 +124,7 @@ struct NodeSlots {
     int B = 0, rowcap = 0, G = 0, steps = 0, key = -1;
     TabDev *d_T = nullptr;
     Rec *d_rec = nullptr;
-    double *M = nullptr, *M2 = nullptr, *prow = nullptr, *pcol = nullptr, *crow = nullptr;
+    double *M = nullptr, *M2 = nullptr, *prow = nullptr, *pcol = nullptr;
     int *vrow = nullptr, *vcol = nullptr;
     Part *part = nullptr;
     int4 *plog = nullptr, *h_logs = nullptr;
@@ -150,7 +137,7 @@ struct NodeSlots {
     void release() {
         if (graph) cudaGraphExecDestroy(graph);
         graph = nullptr;
-        cudaFree(d_T); cudaFree(d_rec); cudaFree(M); cudaFree(M2); cudaFree(prow); cudaFree(pcol); cudaFree(crow);
+        cudaFree(d_T); cudaFree(d_rec); cudaFree(M); cudaFree(M2); cudaFree(prow); cudaFree(pcol);
         cudaFree(vrow); cudaFree(vcol); cudaFree(part); cudaFree(plog);
         cudaFreeHost(h_logs); cudaFreeHost(h_ctl); cudaFreeHost(h_out); cudaFreeHost(h_cuts);
         *this = NodeSlots();

@@ -26,7 +26,7 @@
 //
 // PP = false, the in-place step (two-kernel engine, optional objectives 393-412, very tall tableaux):
 // rank-1 update in place; with do_select the last CTA to finish (atomic ticket) reduces look-ahead partials
-// (cta_tail_lookahead) or runs the generic selection (cta_select<true>).
+// (cta_tail_lookahead) or runs the generic selection (cta_select).
 //
 // Code layout matters as much as instruction count here (DESIGN.md section 6): hot paths are inlined and
 // contiguous, rarely taken ones are __noinline__.
@@ -34,7 +34,7 @@
 // (included inside namespace jslp)
 
 // ---- pricing of the pivot AFTER the staged one (phase 2, no optional objectives) -------------
-// cta_price_scan<true, true> (jslp_kernels.cuh) prices the cost row as the staged pivot will leave
+// cta_price_scan<true> (jslp_kernels.cuh) prices the cost row as the staged pivot will leave
 // it, with the very expression update_rows evaluates for row 0, so the decision is bit-identical
 // to pricing afterwards; one L2 round trip whatever the number of pricing batches.
 
@@ -44,17 +44,16 @@ __device__ __noinline__ void cta_price_next(const TabDev &T, Rec *rec, SelSmem &
     const double q = rec->q;
     const double coef0 = ldg_cg(T.M + cstar);
     int found, neg;
-    cta_price_scan<true, true>(T, s, T.M, T.prow, q, coef0, cstar, T.vcol[cstar], &found, &neg);
+    cta_price_scan<true>(T, s, T.M, T.prow, q, coef0, cstar, T.vcol[cstar], &found, &neg);
     if (threadIdx.x == 0) { rec->next_c = found; rec->next_neg = neg; }
 }
 
-__device__ __forceinline__ double2 upd2(double2 old, double2 f, bool z0, bool z1, double coef, bool pc, int codd,
-                                        double q) {
-    double2 nv = old;
-    if (z0) nv.x = __dsub_rn(old.x, __dmul_rn(coef, f.x));
-    if (z1) nv.y = __dsub_rn(old.y, __dmul_rn(coef, f.y));
+// upd_entry on a column pair of a row with a non-zero pivot-column entry; pc = the pair holds the pivot column (the
+// odd half when codd), whose entry is divided once.
+__device__ __forceinline__ double2 upd2(double2 old, double2 f, double coef, bool pc, int codd, double q) {
+    double2 nv = make_double2(upd_entry(old.x, coef, f.x, false, q), upd_entry(old.y, coef, f.y, false, q));
     if (pc) {
-        const double pv = ddiv(-coef, q);  // simplex.ts:385
+        const double pv = upd_entry(0.0, coef, 0.0, true, q);
         if (codd) nv.y = pv; else nv.x = pv;
     }
     return nv;
@@ -100,7 +99,7 @@ __device__ __noinline__ void update_rows(const TabDev &T, const double *frow, in
                     if (act[j]) old[j] = ld_v2(base + j * stride + 2 * c2);
 #pragma unroll
                 for (int j = 0; j < RC; j++)
-                    if (act[j]) st_v2(base + j * stride + 2 * c2, upd2(old[j], f, z0, z1, coef[j], pc, codd, q));
+                    if (act[j]) st_v2(base + j * stride + 2 * c2, upd2(old[j], f, coef[j], pc, codd, q));
             }
         } else if (any) {
             int c2 = tid;
@@ -125,7 +124,7 @@ __device__ __noinline__ void update_rows(const TabDev &T, const double *frow, in
                 if (z0 || z1 || pc) {
 #pragma unroll
                     for (int j = 0; j < RC; j++)
-                        if (act[j]) st_v2(base + j * stride + 2 * c2, upd2(old[j], f, z0, z1, coef[j], pc, codd, q));
+                        if (act[j]) st_v2(base + j * stride + 2 * c2, upd2(old[j], f, coef[j], pc, codd, q));
                 }
                 c2 = n2;
                 f = fn;
@@ -156,38 +155,17 @@ __device__ __noinline__ void update_rows(const TabDev &T, const double *frow, in
 }
 
 
-// Entry (r, c) of the tableau as the pivot (rstar, cstar, q) leaves it, from its old value: the
-// single-element form of update_rows (simplex.ts:352-391), used to run the look-ahead ratio test on
-// values that were loaded while the pivot row was still being staged.
-__device__ __forceinline__ double new_entry(double old, bool is_prow, double coef, double f, bool is_pc, double q) {
-    if (is_prow) return f;
-    if (nz16(coef)) {
-        if (is_pc) return ddiv(-coef, q);
-        return nz16(f) ? __dsub_rn(old, __dmul_rn(coef, f)) : old;
-    }
-    return old;  // |coef| <= 1e-16: the row is untouched, its pivot-column entry included (simplex.ts:371,389-391 dead)
-}
-
 // ---- look-ahead: ratio-test partial of this CTA's rows against the next entering column ---------
 // One row per thread (nr <= blockDim.x); col/rhs are the UPDATED entries of that row.
 __device__ __forceinline__ void cta_ratio_partial(const TabDev &T, SelSmem &s, int r0, int nr, bool have, double col,
                                                   double rhs, int isneg) {
     const int tid = threadIdx.x;
-    const double prec = T.prec;
-    const VI init = {INFINITY, INT_MAX};
-    VI m = init;
+    VI m = {INFINITY, INT_MAX};
     int dmin = INT_MAX, cnt = 0;
     if (have) {
         const int r = r0 + tid;
         T.pcol[r] = col;  // pivot column of the next pivot (this CTA is the only reader of these entries)
-        if (nz16(col)) cnt = 1;
-        if (r != 0 && !(-prec < col && col < prec)) {
-            if (col > 0 && prec > rhs && rhs > -prec) dmin = r;
-            else {
-                const double quo = ddiv(isneg ? -rhs : rhs, col);
-                if (quo > prec && m.v > quo) { m.v = quo; m.i = r; }
-            }
-        }
+        ratio_step(r, col, rhs, isneg, T.prec, dmin, m, cnt);
     }
     block_reduce_ratio(dmin, m, cnt, s.red);
     const int dall = dmin;
@@ -250,19 +228,12 @@ __device__ __noinline__ void cta_tail_lookahead(const TabDev &T, Rec *rec, SelSm
     const double coef0 = ldg_cg(T.M + cn);
     const int leaving = T.vrow[rstar];
     const int entering = T.vcol[cn];
-    cta_copy_row<true>(T.prow, rowp, T.W, T.stride);
+    cta_copy_row(T.prow, rowp, T.W, T.stride);
     int found, neg;
-    cta_price_scan<true, true>(T, s, T.M, rowp, q, coef0, cn, leaving, &found, &neg);
+    cta_price_scan<true>(T, s, T.M, rowp, q, coef0, cn, leaving, &found, &neg);
     if (tid == 0) {
-        if (log_n < T.plog_cap) T.plog[log_n] = make_int4(rstar | (1 << 30), cn, leaving, entering);
-        rec->log_n = log_n + 1;
-        T.vrow[rstar] = entering;  // simplex.ts:339-349
-        T.vcol[cn] = leaving;
-        rec->phase = 2; rec->r = rstar; rec->c = cn; rec->q = q; rec->is_neg = isneg;
-        rec->flush = (cnt - (nz16(q) ? 1 : 0)) > 0;
-        rec->has_pivot = 1;
-        rec->next_c = found; rec->next_neg = neg;
-        rec->prow_norm = 0;
+        stage_pivot(T, rec, log_n, 2, rstar, cn, leaving, entering, q, isneg, flush_flag(cnt, q), found, 0);
+        rec->next_neg = neg;
     }
 }
 
@@ -300,14 +271,13 @@ __device__ __forceinline__ void update_rows_pp(const double *src, double *dst, i
         const double *sb = src + (size_t)rb * stride;
         double *db = dst + (size_t)rb * stride;
         auto emit = [&](int c2, const double2 f, const double2 *old) {
-            const bool z0 = nz16(f.x), z1 = nz16(f.y);
             const bool pc = (c2 == cpair);
 #pragma unroll
             for (int j = 0; j < RC; j++) {
                 if (!valid[j]) continue;
                 double2 nv;
                 if (isp[j]) nv = f;                                                   // normalised pivot row
-                else if (act[j]) nv = upd2(old[j], f, z0, z1, coef[j], pc, codd, q);  // rank-1 update
+                else if (act[j]) nv = upd2(old[j], f, coef[j], pc, codd, q);  // rank-1 update
                 else nv = old[j];  // untouched row, tiny pivot-column entry included (simplex.ts:371; :389-391 is dead)
                 st_v2(db + j * stride + 2 * c2, nv);
             }
@@ -385,7 +355,7 @@ __device__ __forceinline__ void update_rows_pp_flat(const double *src, double *d
                 if (row == prel) nv = f;  // normalised pivot row
                 else {
                     const double coef = s_coef[row];
-                    nv = nz16(coef) ? upd2(cur[j], f, nz16(f.x), nz16(f.y), coef, c2 == cpair, codd, q) : cur[j];
+                    nv = nz16(coef) ? upd2(cur[j], f, coef, c2 == cpair, codd, q) : cur[j];
                 }
                 st_v2(db + 2 * (size_t)idx, nv);
             }
@@ -540,7 +510,6 @@ __device__ __forceinline__ void cta_selector_decide(TabDev *Tp, const TabDev &T,
     }
     const double qn = new_entry(rv_cn, is_prow, coef_r, frow[cn], cn == cstar, q);      // next pivot element
     const double coef0n = new_entry(cv_cn, false, coef0, frow[cn], cn == cstar, q);     // its cost-row entry
-    const bool nzc = nz16(coef0n);
     const int bsz = T.use_partial ? T.batch_size : max(1, T.W - 1);
     // batches that lie entirely inside the first pass (columns 1 .. K1*NT-1)
     const int covered = min(T.W - 1, K1 * NT - 1);
@@ -555,7 +524,7 @@ __device__ __forceinline__ void cta_selector_decide(TabDev *Tp, const TabDev &T,
             if (c1 >= 1 && c1 < T.W && (c1 - 1) / bsz < nfull) {
                 const double ur = new_entry(rv1[k], is_prow, coef_r, frow[c1], c1 == cstar, q);
                 const double uc = new_entry(cv1[k], false, coef0, frow[c1], c1 == cstar, q);
-                const double nc = priced_cost(uc, ur, coef0n, nzc, c1 == cn, qn);
+                const double nc = priced_cost(uc, ur, coef0n, c1 == cn, qn);
                 int label = -1;
                 if (T.unres != nullptr && nc < 0) label = (c1 == cn) ? leaving : T.vcol[c1];
                 price_consider(T, acc, c1, nc, label, bsz);
@@ -581,7 +550,7 @@ __device__ __forceinline__ void cta_selector_decide(TabDev *Tp, const TabDev &T,
                 if (c >= T.W) continue;
                 const double ur = new_entry(rv[k], is_prow, coef_r, frow[c], c == cstar, q);
                 const double uc = new_entry(cv[k], false, coef0, frow[c], c == cstar, q);
-                const double nc = priced_cost(uc, ur, coef0n, nzc, c == cn, qn);
+                const double nc = priced_cost(uc, ur, coef0n, c == cn, qn);
                 int label = -1;
                 if (T.unres != nullptr && nc < 0) label = (c == cn) ? leaving : T.vcol[c];
                 price_consider(T, acc, c, nc, label, bsz);
@@ -590,16 +559,10 @@ __device__ __forceinline__ void cta_selector_decide(TabDev *Tp, const TabDev &T,
         price_finish_rx(T, s, acc, &found, &neg);
     }
     if (tid == 0) {
-        if (log_n < T.plog_cap) T.plog[log_n] = make_int4(rnext | (1 << 30), cn, leaving, entering);
-        rec->log_n = log_n + 1;
-        T.vrow[rnext] = entering;  // simplex.ts:339-349
-        T.vcol[cn] = leaving;
+        // the staging selector writes the normalised row
+        stage_pivot(T, rec, log_n, 2, rnext, cn, leaving, entering, qn, isneg, flush_flag(cnt, qn), found, 1);
+        rec->next_neg = neg;
         rec->done = launch + 1; rec->p2 = p2 + 1;
-        rec->phase = 2; rec->r = rnext; rec->c = cn; rec->q = qn; rec->is_neg = isneg;
-        rec->flush = (cnt - (nz16(qn) ? 1 : 0)) > 0;
-        rec->has_pivot = 1;
-        rec->next_c = found; rec->next_neg = neg;
-        rec->prow_norm = 1;  // the staging selector writes the normalised row
         flip();
     }
 }
@@ -613,6 +576,35 @@ __device__ __forceinline__ void part_wait(const Part *slot, unsigned int seq) {
         __nanosleep(20);
         if (clock64() - tstart > 4000000000LL) break;
     }
+}
+
+// Stages the NEXT pivot (rnext, cn) for the launch after this one: its row as the executing pivot (rstar, cstar, q,
+// normalised row frow) leaves it, derived from the old tableau (new_entry) and already normalised (norm_entry), so
+// that no CTA of the next launch divides it again, goes into the prow side buffer, zero padded.  cnt = non-zero
+// entries of the next pivot column.  Returns the next pivot element.
+__device__ __forceinline__ double stage_next_row(const TabDev &T, const double *frow, int rstar, int cstar, double q,
+                                                 int rnext, int cn, int cnt) {
+    const int tid = threadIdx.x, NT = blockDim.x;
+    const double *rowp = T.M + (size_t)rnext * T.stride;
+    const bool is_prow = rnext == rstar;
+    const double coef_r = is_prow ? 0.0 : ldg_cg(rowp + cstar);
+    const double qn = new_entry(ldg_cg(rowp + cn), is_prow, coef_r, frow[cn], cn == cstar, q);
+    const bool flushn = flush_flag(cnt, qn);
+    for (int c0 = 0; c0 < T.stride; c0 += 8 * NT) {
+        double rv[8];
+#pragma unroll
+        for (int k = 0; k < 8; k++) {
+            const int c = c0 + tid + k * NT;
+            rv[k] = c < T.W ? ldg_cg(rowp + c) : 0.0;
+        }
+#pragma unroll
+        for (int k = 0; k < 8; k++) {
+            const int c = c0 + tid + k * NT;
+            if (c >= T.stride) continue;
+            T.prow[c] = c < T.W ? norm_entry(new_entry(rv[k], is_prow, coef_r, frow[c], c == cstar, q), c == cn, qn, flushn) : 0.0;
+        }
+    }
+    return qn;
 }
 
 // Selector of a ping-pong step that executes a PHASE-1 pivot (rstar, cstar, q), or a phase-2 pivot whose
@@ -663,6 +655,26 @@ __device__ __noinline__ void cta_selector_decide_full(TabDev *Tp, const TabDev &
     }
     int phase_next = 1, cn = 0, isneg = 0, cnt = 0;
     const bool has_unres = T.unres != nullptr;
+    // non-zero entries of the next pivot column cn as this pivot leaves it (all rows, row 0 included)
+    auto count_col = [&]() {
+        const double f_cn = frow[cn];
+        int n = 0;
+        for (int rb = 0; rb < H; rb += 8 * NT) {
+            double a[8], cf[8];
+#pragma unroll
+            for (int k = 0; k < 8; k++) {
+                const int r = rb + tid + k * NT;
+                a[k] = r < H ? ldg_cg(src + (size_t)r * stride + cn) : 0.0;
+                cf[k] = (r < H && r != rstar) ? ldg_cg(src + (size_t)r * stride + cstar) : 0.0;
+            }
+#pragma unroll
+            for (int k = 0; k < 8; k++) {
+                const int r = rb + tid + k * NT;
+                if (r < H && nz16(new_entry(a[k], r == rstar, cf[k], f_cn, cn == cstar, q))) n++;
+            }
+        }
+        return block_reduce_int<1>(n, s.red);
+    };
     if (rnext >= 0 && T.stride <= 8 * NT) {
         // ---- phase 1 goes on, fast path (two L2 round trips after the partials): the whole derived row
         // rnext fits in eight registers per thread, so the entering-column scan (simplex.ts:56-76), the
@@ -685,11 +697,9 @@ __device__ __noinline__ void cta_selector_decide_full(TabDev *Tp, const TabDev &
             const int c = tid + k * NT;
             if (c >= W) continue;
             ur[k] = new_entry(ur[k], is_prow, coef_r, frow[c], c == cstar, q);
-            if (c >= 1 && ((has_unres && is_unres(T, T.vcol[c])) || ur[k] < -prec)) {
-                const double uc = new_entry(cv[k], false, coef0, frow[c], c == cstar, q);
-                const double quo = ddiv(-uc, ur[k]);
-                if (e.v < quo) { e.v = quo; e.i = c; }
-            }
+            if (c >= 1)
+                entering_step(c, ur[k], has_unres && is_unres(T, T.vcol[c]), prec, e,
+                              [&] { return new_entry(cv[k], false, coef0, frow[c], c == cstar, q); });
         }
         e = block_reduce_vi_rx<false>(e, einit, s.red);
         if (e.i == INT_MAX) {  // simplex.ts:73-76
@@ -709,49 +719,17 @@ __device__ __noinline__ void cta_selector_decide_full(TabDev *Tp, const TabDev &
         // cn?  The cost row and the executing pivot's row are witnesses that cost nothing; only when
         // both are zero is the whole column derived and counted.
         bool flushn = nz16(s.bc0) || (rstar != rnext && nz16(frow[cn]));
-        if (!flushn) {
-            const double f_cn = frow[cn];
-            for (int rb = 0; rb < H; rb += 8 * NT) {
-                double a[8], cf[8];
-#pragma unroll
-                for (int k = 0; k < 8; k++) {
-                    const int r = rb + tid + k * NT;
-                    a[k] = r < H ? ldg_cg(src + (size_t)r * stride + cn) : 0.0;
-                    cf[k] = (r < H && r != rstar) ? ldg_cg(src + (size_t)r * stride + cstar) : 0.0;
-                }
-#pragma unroll
-                for (int k = 0; k < 8; k++) {
-                    const int r = rb + tid + k * NT;
-                    if (r < H && nz16(new_entry(a[k], r == rstar, cf[k], f_cn, cn == cstar, q))) cnt++;
-                }
-            }
-            cnt = block_reduce_int<1>(cnt, s.red);
-            flushn = (cnt - (nz16(qn) ? 1 : 0)) > 0;
-        }
+        if (!flushn) flushn = flush_flag(count_col(), qn);
         const int entering = T.vcol[cn];
 #pragma unroll
         for (int k = 0; k < 8; k++) {
             const int c = tid + k * NT;
-            if (c >= T.stride) continue;
-            double f = 0.0;
-            if (c < W) {
-                f = (c == cn || nz16(ur[k])) ? ddiv(c == cn ? 1.0 : ur[k], qn) : 0.0;
-                if (flushn && !nz16(f) && f != 0.0) f = 0.0;
-            }
-            T.prow[c] = f;
+            if (c < T.stride) T.prow[c] = c < W ? norm_entry(ur[k], c == cn, qn, flushn) : 0.0;
         }
         __syncthreads();
         if (tid == 0) {
-            if (log_n < T.plog_cap) T.plog[log_n] = make_int4(rnext, cn, leaving, entering);
-            rec->log_n = log_n + 1;
-            T.vrow[rnext] = entering;  // simplex.ts:339-349
-            T.vcol[cn] = leaving;
+            stage_pivot(T, rec, log_n, 1, rnext, cn, leaving, entering, qn, 0, flushn, -1, 1);
             rec->done = launch + 1; rec->p1 = pcount + 1;
-            rec->phase = 1; rec->r = rnext; rec->c = cn; rec->q = qn; rec->is_neg = 0;
-            rec->flush = flushn ? 1 : 0;
-            rec->has_pivot = 1;
-            rec->next_c = -1;    // the pivot after this one has not been priced
-            rec->prow_norm = 1;  // the row above is already normalised
             __threadfence();     // prow and the record are read by the next launch
             flip();
         }
@@ -776,12 +754,9 @@ __device__ __noinline__ void cta_selector_decide_full(TabDev *Tp, const TabDev &
             for (int k = 0; k < 8; k++) {
                 const int c = c0 + tid + k * NT;
                 if (c >= W) continue;
-                const double ur = new_entry(rv[k], is_prow, coef_r, frow[c], c == cstar, q);
-                if ((has_unres && is_unres(T, T.vcol[c])) || ur < -prec) {
-                    const double uc = new_entry(cv[k], false, coef0, frow[c], c == cstar, q);
-                    const double quo = ddiv(-uc, ur);
-                    if (e.v < quo) { e.v = quo; e.i = c; }
-                }
+                entering_step(c, new_entry(rv[k], is_prow, coef_r, frow[c], c == cstar, q),
+                              has_unres && is_unres(T, T.vcol[c]), prec, e,
+                              [&] { return new_entry(cv[k], false, coef0, frow[c], c == cstar, q); });
             }
         }
         e = block_reduce_vi_rx<false>(e, einit, s.red);
@@ -790,23 +765,7 @@ __device__ __noinline__ void cta_selector_decide_full(TabDev *Tp, const TabDev &
             return;
         }
         cn = e.i;
-        // non-zero entries of the next pivot column as this pivot leaves it (all rows, incl. row 0)
-        const double f_cn = frow[cn];
-        for (int rb = 0; rb < H; rb += 8 * NT) {
-            double a[8], cf[8];
-#pragma unroll
-            for (int k = 0; k < 8; k++) {
-                const int r = rb + tid + k * NT;
-                a[k] = r < H ? ldg_cg(src + (size_t)r * stride + cn) : 0.0;
-                cf[k] = (r < H && r != rstar) ? ldg_cg(src + (size_t)r * stride + cstar) : 0.0;
-            }
-#pragma unroll
-            for (int k = 0; k < 8; k++) {
-                const int r = rb + tid + k * NT;
-                if (r < H && nz16(new_entry(a[k], r == rstar, cf[k], f_cn, cn == cstar, q))) cnt++;
-            }
-        }
-        cnt = block_reduce_int<1>(cnt, s.red);
+        cnt = count_col();
     } else {
         // ---- feasible after this pivot (simplex.ts:51-54), or already in phase 2
         if (phase_exec == 1 && only_phase == 1) {
@@ -843,8 +802,7 @@ __device__ __noinline__ void cta_selector_decide_full(TabDev *Tp, const TabDev &
             return;
         }
         // ratio test (simplex.ts:271-296) on the derived pivot column and right-hand side
-        const VI init = {INFINITY, INT_MAX};
-        VI m = init;
+        VI m = {INFINITY, INT_MAX};
         int dmin = INT_MAX;
         const double f_cn = frow[cn], f_0 = frow[0];
         for (int rb = 0; rb < H; rb += 8 * NT) {
@@ -861,14 +819,8 @@ __device__ __noinline__ void cta_selector_decide_full(TabDev *Tp, const TabDev &
                 const int r = rb + tid + k * NT;
                 if (r >= H) continue;
                 const double col = new_entry(a[k], r == rstar, cf[k], f_cn, cn == cstar, q);
-                const double rhs = new_entry(b0[k], r == rstar, cf[k], f_0, false, q);
                 T.pcol[r] = col;  // the step that executes this pivot runs in place and reads its column here
-                if (nz16(col)) cnt++;
-                if (r == 0) continue;
-                if (-prec < col && col < prec) continue;
-                if (col > 0 && prec > rhs && rhs > -prec) { dmin = min(dmin, r); continue; }
-                const double quo = ddiv(isneg ? -rhs : rhs, col);
-                if (quo > prec && m.v > quo) { m.v = quo; m.i = r; }
+                ratio_step(r, col, new_entry(b0[k], r == rstar, cf[k], f_0, false, q), isneg, prec, dmin, m, cnt);
             }
         }
         { int okd = 1; block_reduce_ratio_rx(dmin, m, cnt, okd, s.red); }
@@ -880,100 +832,32 @@ __device__ __noinline__ void cta_selector_decide_full(TabDev *Tp, const TabDev &
         }
     }
     // ---- stage pivot (rnext, cn): normalised row into the prow side buffer, labels, log, record
-    const double *rowp = src + (size_t)rnext * stride;
-    const bool is_prow = rnext == rstar;
-    const double coef_r = is_prow ? 0.0 : ldg_cg(rowp + cstar);
-    const double qn = new_entry(ldg_cg(rowp + cn), is_prow, coef_r, frow[cn], cn == cstar, q);
-    const bool flushn = (cnt - (nz16(qn) ? 1 : 0)) > 0;
     const int leaving = T.vrow[rnext];
     const int entering = T.vcol[cn];
     __syncthreads();
-    for (int c0 = 0; c0 < T.stride; c0 += 8 * NT) {
-        double rv[8];
-#pragma unroll
-        for (int k = 0; k < 8; k++) {
-            const int c = c0 + tid + k * NT;
-            rv[k] = c < W ? ldg_cg(rowp + c) : 0.0;
-        }
-#pragma unroll
-        for (int k = 0; k < 8; k++) {
-            const int c = c0 + tid + k * NT;
-            if (c >= T.stride) continue;
-            double f = 0.0;
-            if (c < W) {
-                const double ur = new_entry(rv[k], is_prow, coef_r, frow[c], c == cstar, q);
-                f = (c == cn || nz16(ur)) ? ddiv(c == cn ? 1.0 : ur, qn) : 0.0;
-                if (flushn && !nz16(f) && f != 0.0) f = 0.0;
-            }
-            T.prow[c] = f;
-        }
-    }
+    const double qn = stage_next_row(T, frow, rstar, cstar, q, rnext, cn, cnt);
     __syncthreads();
     if (tid == 0) {
-        if (log_n < T.plog_cap) T.plog[log_n] = make_int4(rnext | (phase_next == 2 ? (1 << 30) : 0), cn, leaving, entering);
-        rec->log_n = log_n + 1;
-        T.vrow[rnext] = entering;  // simplex.ts:339-349
-        T.vcol[cn] = leaving;
+        stage_pivot(T, rec, log_n, phase_next, rnext, cn, leaving, entering, qn, isneg, flush_flag(cnt, qn), -1, 1);
         rec->done = launch + 1;
         if (phase_exec == 1) rec->p1 = pcount + 1; else rec->p2 = pcount + 1;
-        rec->phase = phase_next; rec->r = rnext; rec->c = cn; rec->q = qn; rec->is_neg = isneg;
-        rec->flush = flushn;
-        rec->has_pivot = 1;
-        rec->next_c = -1;    // the pivot after this one has not been priced
-        rec->prow_norm = 1;  // the row above is already normalised
         __threadfence();     // prow and the record are read by the next launch
         flip();
     }
 }
 
-// Selector S2 of a ping-pong step: stages the raw pivot row of the next pivot (the row as the
-// executing pivot leaves it) into the prow side buffer, the TMA source of the next launch.
-__device__ __forceinline__ void cta_selector_stage(const TabDev &T, Rec *rec, SelSmem &s, const double *frow, int G, int rstar,
+// Selector S2 of a ping-pong step: stages the next pivot row (the row as the executing pivot leaves it, already
+// normalised) into the prow side buffer, the TMA source of the next launch.
+__device__ __forceinline__ void cta_selector_stage(const TabDev &T, SelSmem &s, const double *frow, int G, int rstar,
                                    int cstar, double q, int cn, int launch, bool stop_after) {
-    const int tid = threadIdx.x, NT = blockDim.x;
     if (cn == 0 || stop_after) return;
     int rnext, cnt;
     if (!cta_collect_partials(T, s, G, (unsigned int)(launch + 1), &rnext, &cnt)) return;  // S1 reports the error
     if (rnext < 0) return;
-    if (tid == 0) {  // the other selector must also be done reading the prow buffer (slot G is its message)
-        double dq;
-        int d1, d2, d3;
-        const long long tstart = clock64();
-        while (!part_try_read(T.part + G, (unsigned int)(launch + 1), &dq, &d1, &d2, &d3)) {
-            __nanosleep(20);
-            if (clock64() - tstart > 4000000000LL) break;
-        }
-    }
+    // the other selector must also be done reading the prow buffer (slot G is its message)
+    if (threadIdx.x == 0) part_wait(T.part + G, (unsigned int)(launch + 1));
     __syncthreads();
-    const double *src = T.M;
-    const double *rowp = src + (size_t)rnext * T.stride;
-    const bool is_prow = rnext == rstar;
-    const double coef_r = is_prow ? 0.0 : ldg_cg(rowp + cstar);
-    // pivot element and lazy-flush flag of the next pivot: the row is staged already NORMALISED
-    // (simplex.ts:352-364, 380-382), so no CTA of the next launch has to divide it again
-    const double qn = new_entry(ldg_cg(rowp + cn), is_prow, coef_r, frow[cn], cn == cstar, q);
-    const bool flushn = (cnt - (nz16(qn) ? 1 : 0)) > 0;
-    for (int c0 = 0; c0 < T.stride; c0 += 8 * NT) {
-        double rv[8];
-#pragma unroll
-        for (int k = 0; k < 8; k++) {
-            const int c = c0 + tid + k * NT;
-            rv[k] = c < T.W ? ldg_cg(rowp + c) : 0.0;
-        }
-#pragma unroll
-        for (int k = 0; k < 8; k++) {
-            const int c = c0 + tid + k * NT;
-            if (c >= T.stride) continue;
-            double f = 0.0;
-            if (c < T.W) {
-                const double ur = new_entry(rv[k], is_prow, coef_r, frow[c], c == cstar, q);
-                f = (c == cn || nz16(ur)) ? ddiv(c == cn ? 1.0 : ur, qn) : 0.0;
-                if (flushn && !nz16(f) && f != 0.0) f = 0.0;
-            }
-            T.prow[c] = f;
-        }
-    }
-    (void)rec;
+    stage_next_row(T, frow, rstar, cstar, q, rnext, cn, cnt);
 }
 
 // ---- the kernel ------------------------------------------------------------------------------------
@@ -1077,11 +961,7 @@ __global__ void __launch_bounds__(NTHREADS, MINB)
             if (lane < nr) s_coef[lane] = la_coef;
             if (want_partial && pp1) {
                 // phase 1: the most negative right-hand side of this CTA's rows after this pivot
-                double f_0 = raw_0;
-                if (!prow_norm) {
-                    f_0 = nz16(raw_0) ? ddiv(raw_0, q) : 0.0;
-                    if (flush && !nz16(f_0) && f_0 != 0.0) f_0 = 0.0;
-                }
+                const double f_0 = prow_norm ? raw_0 : norm_entry(raw_0, false, q, flush);
                 const bool is_prow = (r0 + lane) == rstar;
                 const double rhs = new_entry(la_rhs, is_prow, la_coef, f_0, false, q);
                 VI m = {INFINITY, INT_MAX};
@@ -1093,50 +973,28 @@ __global__ void __launch_bounds__(NTHREADS, MINB)
                     if (dbg) T.dbg[((size_t)launch * T.dbg_grid + b) * 8 + 2] = clock64() - s_t0;
                 }
             } else if (want_partial) {
-                double f_n = raw_n, f_0 = raw_0;
-                if (!prow_norm) {
-                    f_n = (next_c == cstar || nz16(raw_n)) ? ddiv(next_c == cstar ? 1.0 : raw_n, q) : 0.0;
-                    if (flush && !nz16(f_n) && f_n != 0.0) f_n = 0.0;
-                    f_0 = nz16(raw_0) ? ddiv(raw_0, q) : 0.0;
-                    if (flush && !nz16(f_0) && f_0 != 0.0) f_0 = 0.0;
-                }
+                const double f_n = prow_norm ? raw_n : norm_entry(raw_n, next_c == cstar, q, flush);
+                const double f_0 = prow_norm ? raw_0 : norm_entry(raw_0, false, q, flush);
                 const bool is_prow = (r0 + lane) == rstar;
                 const double col = new_entry(la_col, is_prow, la_coef, f_n, next_c == cstar, q);
                 const double rhs = new_entry(la_rhs, is_prow, la_coef, f_0, false, q);
-                const double prec = T.prec;
                 VI m = {INFINITY, INT_MAX};
                 int dmin = INT_MAX, cnt = 0;
-                if (lane < nr) {
-                    const int r = r0 + lane;
-                    if (nz16(col)) cnt = 1;
-                    if (r != 0 && !(-prec < col && col < prec)) {
-                        if (col > 0 && prec > rhs && rhs > -prec) dmin = lane;
-                        else {
-                            const double quo = ddiv(next_neg ? -rhs : rhs, col);
-                            if (quo > prec && m.v > quo) { m.v = quo; m.i = lane; }
-                        }
-                    }
-                }
+                if (lane < nr) ratio_step(r0 + lane, col, rhs, next_neg, T.prec, dmin, m, cnt);
                 m = warp_reduce_vi<true>(m);
                 dmin = __reduce_min_sync(0xffffffffu, dmin);
                 cnt = __reduce_add_sync(0xffffffffu, cnt);
-                if (lane == 0) {
+                if (lane == 0) {  // rows go out relative to r0
                     mbar_wait(&bar, 0);  // a published partial also promises: this CTA is done reading prow
-                    part_publish(T.part + b, m.v, m.i == INT_MAX ? 255 : m.i, dmin == INT_MAX ? 255 : dmin, cnt,
+                    part_publish(T.part + b, m.v, m.i == INT_MAX ? 255 : m.i - r0, dmin == INT_MAX ? 255 : dmin - r0, cnt,
                                  (unsigned int)(launch + 1));
                     if (dbg) T.dbg[((size_t)launch * T.dbg_grid + b) * 8 + 2] = clock64() - s_t0;
                 }
             }
         }
         mbar_wait(&bar, 0);
-        if (!prow_norm) {
-            for (int c = tid; c < T.stride; c += NT) {  // normalise (simplex.ts:352-364, 380-382)
-                const double v = frow[c];
-                double f = (c == cstar || nz16(v)) ? ddiv(c == cstar ? 1.0 : v, q) : 0.0;
-                if (flush && !nz16(f) && f != 0.0) f = 0.0;
-                frow[c] = f;
-            }
-        }
+        if (!prow_norm)
+            for (int c = tid; c < T.stride; c += NT) frow[c] = norm_entry(frow[c], c == cstar, q, flush);
         __syncthreads();
         if (dbg && tid == 0) t1 = clock64();
         if (!pp2 && b == G) {
@@ -1154,7 +1012,7 @@ __global__ void __launch_bounds__(NTHREADS, MINB)
             cta_selector_decide(Tp, T, rec, sel, frow, G, rstar, cstar, q, next_c, next_neg, launch, p2, log_n0, stop_after, ts);
             if (dbg && tid == 0) { t2 = ts[0]; t3 = ts[1]; g0 = ts[2] - t0; }  // partials in, reduced, first pricing pass
         } else if (b == G + 1) {
-            cta_selector_stage(T, rec, sel, frow, G, rstar, cstar, q, next_c, launch, stop_after);
+            cta_selector_stage(T, sel, frow, G, rstar, cstar, q, next_c, launch, stop_after);
             if (dbg && tid == 0) t2 = t3 = clock64();
         } else {
             if constexpr (RC < 0) update_rows_pp_flat<-RC>(T.M, T.M2, T.stride, frow, s_coef, r0, nr, rstar, cstar, q);
@@ -1185,14 +1043,8 @@ __global__ void __launch_bounds__(NTHREADS, MINB)
     }
 
     mbar_wait(&bar, 0);
-    if (!prow_norm) {
-        for (int c = tid; c < T.stride; c += NT) {  // normalise in place (simplex.ts:352-364, 380-382)
-            const double v = frow[c];
-            double f = (c == cstar || nz16(v)) ? ddiv(c == cstar ? 1.0 : v, q) : 0.0;
-            if (flush && !nz16(f) && f != 0.0) f = 0.0;
-            frow[c] = f;
-        }
-    }
+    if (!prow_norm)
+        for (int c = tid; c < T.stride; c += NT) frow[c] = norm_entry(frow[c], c == cstar, q, flush);
     __syncthreads();
     if (dbg && tid == 0) t1 = clock64();
 
@@ -1227,7 +1079,7 @@ __global__ void __launch_bounds__(NTHREADS, MINB)
                 cta_tail_lookahead(T, rec, sel, G, next_c, next_neg, log_n0);
             } else {
                 __syncthreads();
-                cta_select<true>(T, rec, sel);
+                cta_select(T, rec, sel);
                 __syncthreads();
                 if (lookahead && rec->has_pivot && rec->phase == 2 && T.nOpt == 0) cta_price_next(T, rec, sel);
             }

@@ -150,6 +150,21 @@ def test_mixed_lp_with_phase1(n, m, seed, engine, monkeypatch):
     assert_lp_parity(g, o, f"mixed {n}x{m}")
 
 
+@pytest.mark.parametrize("engine", ["auto", "fused_inplace"])
+def test_wide_mixed_lp_with_phase1(engine):
+    """31 x 2101 tableau: the row stride (2112) exceeds 8 columns x 256 threads, so the ping-pong selector derives the
+    phase-1 entering column with the wide-tableau loop instead of its register-resident fast path."""
+    from jslpsolver_b200 import problems
+    from jslpsolver_b200.model import Model
+    it = Model().loadJson(problems.mixed_lp_model(2100, 30, seed=15)).initial_tableau()
+    o = oracle_lp(it)
+    o.simplex()
+    g = gpu_lp(it, 0 if engine == "auto" else ENGINES[engine])
+    g.simplex()
+    assert_lp_parity(g, o, f"wide mixed 2100x30 {engine}")
+    assert g.lastStatus.phase1_pivots > 0
+
+
 @pytest.mark.parametrize("batch", [1, 2, 3, 7])
 def test_small_batches_and_cycle_rewind(batch):
     """Cycle detection runs on the host over the drained log; with tiny batches the rewind
