@@ -191,6 +191,17 @@ int jslp_download(jslp_tab *tab, double *matrix, double *rhs_col, double *cost_r
 /* Drains the host-side pivot log: 4 int32 per pivot (row, col, leaving var, entering var). */
 int jslp_pivot_log(jslp_tab *tab, int32_t *entries, int cap, int *n);
 
+/* Ratio-test bounds of the current tableau for the sensitivity report of a solved LP (no reference counterpart;
+ * DESIGN.md section 2b).  One device pass over rows 1 .. height-1; the tableau, the index maps and the pivot record are
+ * left unchanged.  With P = precision and only rows / columns as stated taking part:
+ *   col_lo[c] / col_hi[c]  width doubles: max / min of -M[r,0] / M[r,c] over rows whose basic variable is restricted
+ *                          and M[r,c] > P / M[r,c] < -P
+ *   row_lo[r] / row_hi[r]  height doubles: max / min of M[0,c] / M[r,c] over restricted columns c >= 1 with
+ *                          M[r,c] > P / M[r,c] < -P; an unrestricted column with |M[r,c]| > P contributes 0 to both
+ * Quotients are normalised from -0 to +0 and NaN quotients are skipped; an empty set gives -inf (lo) / +inf (hi), as do row 0 and column 0.
+ * Duals and reduced costs are the cost row itself (jslp_download's cost_row). */
+int jslp_sensitivity(jslp_tab *tab, double *col_lo, double *col_hi, double *row_lo, double *row_hi);
+
 /* Multi-GPU communicator of the branch-and-cut frontier (one process per GPU).  NCCL is loaded at run time;
  * without libnccl these calls fail with JSLP_E_UNSUPPORTED and single-GPU use is unaffected.  Rank 0 obtains a
  * 128-byte unique id and hands it to the other ranks through whatever bootstrap the host has (the N-API host:

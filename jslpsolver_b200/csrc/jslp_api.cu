@@ -165,6 +165,8 @@ struct jslp_tab {
     int slot_steps = 32;    // pivots per slot per host poll
     int slot_variant = 12;  // kernel instantiation of the slot batch: flat streaming, 3 CTAs per SM (more row CTAs per slot)
     long long node_kernel_ns = 0;  // sum over rounds of the slowest node CTA (reporting)
+    unsigned long long *d_sens = nullptr;  // jslp_sensitivity's key buffers: 2 x sens_cap
+    size_t sens_cap = 0;
 };
 
 extern "C" const char *jslp_last_error(void) { return g_err.c_str(); }
@@ -329,6 +331,7 @@ extern "C" void jslp_tab_destroy(jslp_tab *t) {
     cudaFree(t->d_T); cudaFree(t->d_rec); cudaFree(t->d_mip); cudaFree(t->d_cuts);
     cudaFreeHost(t->h_rec); cudaFreeHost(t->h_log); cudaFreeHost(t->h_mip); cudaFreeHost(t->h_cuts);
     cudaFree(t->d_count); cudaFreeHost(t->h_count);
+    cudaFree(t->d_sens);
     free_saved(t->saved);
     free_snap(t->snaps[0]);
     free_snap(t->snaps[1]);
@@ -1344,3 +1347,4 @@ extern "C" int jslp_pivot_log(jslp_tab *t, int32_t *entries, int cap, int *n) {
 #include "jslp_comm.cuh"
 #include "jslp_bnb_enhanced.cuh"
 #include "jslp_bnb.cuh"
+#include "jslp_sensitivity.cuh"

@@ -80,6 +80,7 @@ class Constraint:  # expressions.ts:96-203
         self.slack = Variable("s" + str(index), 0, index, 0, isSlack=True)
         self.coef: dict[int, Term] = {}  # var index -> term, insertion ordered
         self.relaxation: Optional[Variable] = None
+        self.name: Optional[str] = None  # the JSON constraint name when loadJson built the row
 
     @property
     def terms(self) -> list[Term]:
@@ -342,15 +343,18 @@ class Model:
             if spec.get("equal") is None:
                 if spec.get("min") is not None:
                     c = by_min[name] = self.greaterThan(spec["min"])
+                    c.name = name
                     if relaxed:
                         c.relax(weight, priority)
                 if spec.get("max") is not None:
                     c = by_max[name] = self.smallerThan(spec["max"])
+                    c.name = name
                     if relaxed:
                         c.relax(weight, priority)
             else:
                 lo = by_min[name] = self.greaterThan(spec["equal"])
                 up = by_max[name] = self.smallerThan(spec["equal"])
+                lo.name = up.name = name
                 if relaxed:
                     Equality(lo, up).relax(weight, priority)
 

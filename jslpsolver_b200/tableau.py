@@ -70,7 +70,14 @@ class Solution:  # solution.ts:16-61
     def __init__(self, tableau: "GpuTableau", evaluation: float, feasible: bool, bounded: bool):
         self.feasible, self.evaluation, self.bounded = feasible, evaluation, bounded
         self._tableau = tableau
+        self._version = getattr(tableau, "_version", None)  # the tableau state this solution describes
         self.solutionSet: dict = {}
+
+    def sensitivity(self) -> dict:
+        """Shadow prices, reduced costs and right-hand-side / cost ranges of this continuous LP optimum
+        (DESIGN.md section 2b); raises ValueError where they are not defined."""
+        from .sensitivity import report
+        return report(self)
 
     def generateSolutionSet(self) -> dict:
         t = self._tableau
@@ -127,6 +134,8 @@ class GpuTableau:
         self.availableIndexes: list = []   # tableau.ts:77
         self._cache: dict = {}
         self._cache_log = None
+        self._version = 0          # bumped by every change of the device tableau (solves and edits)
+        self._solved_version = -1  # _version right after the last simplex()
 
     # name-mangling-free accessor used by Solve (main.ts:180)
     @property
@@ -181,7 +190,7 @@ class GpuTableau:
             self.set_option(_lib.OPT_ENGINE, self.engine)
         for k, v in self.options.items():
             self.set_option(k, v)
-        self._cache.clear()
+        self._edited()
         self._cache_log = None
         return self
 
@@ -195,6 +204,10 @@ class GpuTableau:
 
     def set_option(self, key: int, value: float) -> None:
         _lib.check(self.context.lib.jslp_tab_set_option(self._h(), key, float(value)))
+
+    def _edited(self) -> None:
+        self._cache.clear()
+        self._version += 1
 
     def _h(self):
         if self.handle is None:
@@ -216,13 +229,14 @@ class GpuTableau:
         if st.cycled and self.model is not None:  # simplex.ts:86-88 / 313-315
             self.model.messages += [f"Cycle in phase {st.cycled}", f"Start :{st.cycle_start}",
                                     f"Length :{st.cycle_length}"]
-        self._cache.clear()
+        self._edited()
 
     # ------------------------------------------------------------------ simplex (tableau.ts:103-123)
     def simplex(self) -> "GpuTableau":
         st = LpStatus()
         _lib.check(self.context.lib.jslp_simplex(self._h(), self._check_cycles(), C.byref(st)))
         self._absorb(st)
+        self._solved_version = self._version
         return self
 
     def phase1(self) -> int:
@@ -239,7 +253,7 @@ class GpuTableau:
 
     def pivot(self, pivotRowIndex: int, pivotColumnIndex: int) -> None:
         _lib.check(self.context.lib.jslp_pivot(self._h(), pivotRowIndex, pivotColumnIndex))
-        self._cache.clear()
+        self._edited()
 
     # ------------------------------------------------------------------ backup (tableau.ts:219-229)
     def save(self) -> None:
@@ -253,7 +267,7 @@ class GpuTableau:
         info = (C.c_int32 * 6)()
         _lib.check(self.context.lib.jslp_tab_info(self._h(), info))
         self.width, self.height, self.nVars, self.lastElementIndex = info[0], info[1], info[2], info[3]
-        self._cache.clear()
+        self._edited()
 
     def getNewElementIndex(self) -> int:  # tableau.ts:393-401
         if self.availableIndexes:
@@ -274,19 +288,19 @@ class GpuTableau:
     def putInBase(self, varIndex: int) -> int:
         r = C.c_int()
         _lib.check(self.context.lib.jslp_put_in_base(self._h(), int(varIndex), C.byref(r)))
-        self._cache.clear()
+        self._edited()
         return r.value
 
     def takeOutOfBase(self, varIndex: int) -> int:
         c = C.c_int()
         _lib.check(self.context.lib.jslp_take_out_of_base(self._h(), int(varIndex), C.byref(c)))
-        self._cache.clear()
+        self._edited()
         return c.value
 
     def updateRightHandSide(self, constraint, difference: float) -> None:
         idx = constraint if isinstance(constraint, int) else constraint.index
         _lib.check(self.context.lib.jslp_update_rhs(self._h(), int(idx), float(difference)))
-        self._cache.clear()
+        self._edited()
 
     def updateConstraintCoefficient(self, constraint, variable, difference: float) -> None:
         ci = constraint if isinstance(constraint, int) else constraint.index
@@ -294,13 +308,13 @@ class GpuTableau:
         if ci == vi:  # dynamic-modification.ts:114-118
             raise ValueError("[Tableau.updateConstraintCoefficient] constraint index should not be equal to variable index !")
         _lib.check(self.context.lib.jslp_update_coefficient(self._h(), int(ci), int(vi), float(difference)))
-        self._cache.clear()
+        self._edited()
 
     def updateCost(self, variable, difference: float, priority: int = 0) -> None:
         vi = variable if isinstance(variable, int) else variable.index
         pr = priority if isinstance(variable, int) else variable.priority
         _lib.check(self.context.lib.jslp_update_cost(self._h(), int(vi), self._opt_slot(pr), float(difference)))
-        self._cache.clear()
+        self._edited()
 
     def addConstraint(self, constraint=None, *, isUpperBound=None, rhs=None, index=None, terms=None) -> None:
         if constraint is not None:
@@ -547,6 +561,25 @@ class GpuTableau:
         for c in range(1, len(vc)):
             out[vc[c]] = c
         return out
+
+    def final_state(self):
+        """(right-hand-side column, cost row, varIndexByRow, varIndexByCol) in one read-back."""
+        H, W = self.height, self.width
+        rhs, cost = np.empty(H, dtype=np.float64), np.empty(W, dtype=np.float64)
+        vr, vc = np.empty(H, dtype=np.int32), np.empty(W, dtype=np.int32)
+        _lib.check(self.context.lib.jslp_download(self._h(), None, rhs.ctypes.data, cost.ctypes.data, vr.ctypes.data,
+                                                  vc.ctypes.data, None, None, None))
+        return rhs, cost, vr, vc
+
+    def sensitivity_bounds(self):
+        """jslp_sensitivity: (col_lo, col_hi) over the columns and (row_lo, row_hi) over the rows of the current
+        tableau, the ratio-test bounds the sensitivity report is built from (DESIGN.md section 2b)."""
+        H, W = self.height, self.width
+        col_lo, col_hi = np.empty(W, dtype=np.float64), np.empty(W, dtype=np.float64)
+        row_lo, row_hi = np.empty(H, dtype=np.float64), np.empty(H, dtype=np.float64)
+        _lib.check(self.context.lib.jslp_sensitivity(self._h(), col_lo.ctypes.data, col_hi.ctypes.data,
+                                                     row_lo.ctypes.data, row_hi.ctypes.data))
+        return col_lo, col_hi, row_lo, row_hi
 
     def optional_reduced_costs(self) -> np.ndarray:
         return self._download("opt")
