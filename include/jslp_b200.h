@@ -202,6 +202,12 @@ int jslp_pivot_log(jslp_tab *tab, int32_t *entries, int cap, int *n);
  * Duals and reduced costs are the cost row itself (jslp_download's cost_row). */
 int jslp_sensitivity(jslp_tab *tab, double *col_lo, double *col_hi, double *row_lo, double *row_hi);
 
+/* Phase-1 feasibility of row subsets of the tableau's saved snapshot (jslp_save); no reference counterpart,
+ * DESIGN.md section 2c.  keep: n_sets * height bytes, keep[s*height + r] = 1 keeps row r in set s (row 0 is
+ * always kept).  verdict[s]: 0 = feasible, 1 = infeasible, 2 = undecided (cycle).  pivots[s] (may be NULL):
+ * phase-1 pivots.  The cycle check is always on.  On return the tableau equals its snapshot. */
+int jslp_feasibility_batch(jslp_tab *tab, const uint8_t *keep, int n_sets, int32_t *verdict, int32_t *pivots);
+
 /* Multi-GPU communicator of the branch-and-cut frontier (one process per GPU).  NCCL is loaded at run time;
  * without libnccl these calls fail with JSLP_E_UNSUPPORTED and single-GPU use is unaffected.  Rank 0 obtains a
  * 128-byte unique id and hands it to the other ranks through whatever bootstrap the host has (the N-API host:

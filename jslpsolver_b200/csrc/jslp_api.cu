@@ -167,6 +167,8 @@ struct jslp_tab {
     long long node_kernel_ns = 0;  // sum over rounds of the slowest node CTA (reporting)
     unsigned long long *d_sens = nullptr;  // jslp_sensitivity's key buffers: 2 x sens_cap
     size_t sens_cap = 0;
+    void *d_iis = nullptr;  // jslp_feasibility_batch: packed keep masks / the gathered row list
+    size_t iis_bytes = 0;
 };
 
 extern "C" const char *jslp_last_error(void) { return g_err.c_str(); }
@@ -331,7 +333,7 @@ extern "C" void jslp_tab_destroy(jslp_tab *t) {
     cudaFree(t->d_T); cudaFree(t->d_rec); cudaFree(t->d_mip); cudaFree(t->d_cuts);
     cudaFreeHost(t->h_rec); cudaFreeHost(t->h_log); cudaFreeHost(t->h_mip); cudaFreeHost(t->h_cuts);
     cudaFree(t->d_count); cudaFreeHost(t->h_count);
-    cudaFree(t->d_sens);
+    cudaFree(t->d_sens); cudaFree(t->d_iis);
     free_saved(t->saved);
     free_snap(t->snaps[0]);
     free_snap(t->snaps[1]);
@@ -807,10 +809,10 @@ static int run_lp_resident(jslp_tab *t, int check_cycles, jslp_lp_status *out, b
     nb.H0 = t->H; nb.root_stride = t->stride; nb.first_index = t->lastElementIndex;
     nb.Hcap = t->H; nb.Ws = Ws; nb.log_cap = log_cap; nb.max_pivots = log_cap - 2;
     if ((int)smem > rb.smem_set) {
-        CK(cudaFuncSetAttribute(k_node_batch, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CK(cudaFuncSetAttribute(k_node_batch<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         rb.smem_set = (int)smem;
     }
-    k_node_batch<<<1, NODE_THREADS, smem, s>>>(t->d_T, nb);
+    k_node_batch<false><<<1, NODE_THREADS, smem, s>>>(t->d_T, nb);
     ctx->launches += 1;
     CK(cudaGetLastError());
     CK(cudaStreamSynchronize(s));
@@ -1348,3 +1350,4 @@ extern "C" int jslp_pivot_log(jslp_tab *t, int32_t *entries, int cap, int *n) {
 #include "jslp_bnb_enhanced.cuh"
 #include "jslp_bnb.cuh"
 #include "jslp_sensitivity.cuh"
+#include "jslp_iis.cuh"

@@ -48,6 +48,11 @@ struct NodeBatchDev {
     double *wb_M;          // optional write-back of node 0's final tableau (stride = root_stride)
     int *wb_vrow, *wb_vcol;
     int H0, root_stride, first_index, Hcap, Ws, log_cap, max_pivots;
+    // row-subset launches (k_node_batch<true>, jslp_feasibility_batch): node n keeps the root rows whose bits are set
+    // in keep[n * keep_words ...] (device memory; row 0 is always kept), and with phase1_only the CTA stops with
+    // ST_P1_DONE where phase 1 finds no leaving row.  Not read by k_node_batch<false>.
+    const uint32_t *keep;
+    int keep_words, phase1_only;
     int n_inline;          // > 0: cut_off_inline holds the n_inline + 1 offsets (saves a PCIe round trip)
     int cut_off_inline[NODE_INLINE_OFF + 1];
 };
@@ -107,6 +112,11 @@ struct NodePart {    // per-warp partial results of a scan
     int i[8], d[8], n[8];
 };
 
+// SUBSET = false: branch-and-cut nodes and engine 4 (every root row, then the node's cuts).  SUBSET = true: one row
+// subset of the root per CTA (NodeBatchDev.keep), compacted in row order; row labels stay the root's, so the
+// unrestricted lookup and the pivot log read as on the whole tableau.  A template parameter, so that the node path
+// carries none of the subset code.
+template <bool SUBSET>
 __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, const __grid_constant__ NodeBatchDev nb) {
     extern __shared__ __align__(16) unsigned char smraw[];
     __shared__ TabDev T;
@@ -115,7 +125,7 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
     __shared__ NodePivot piv;
     __shared__ NodeScan sc;
     __shared__ NodePart part;
-    __shared__ int s_spare;
+    __shared__ int s_spare, s_kept;
     __shared__ int s_fin[8];   // status, p1, p2, log_n, overflow, unbounded_var
     __shared__ double s_eval;
     __shared__ __align__(8) uint64_t s_bar;
@@ -143,11 +153,32 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
         fence_mbar_init();
     }
     __syncthreads();
+    int H0k = H0;  // rows restored from the root
+    if constexpr (SUBSET) {
+        // compacted position of every kept row: slot[d] = the root row that becomes row d (slot is reset below,
+        // once the copies that read it have been issued)
+        if (warp == 0) {
+            const uint32_t *kw = nb.keep + (size_t)node * nb.keep_words;
+            int base = 0;
+            for (int r0 = 0; r0 < H0; r0 += 32) {
+                const int r = r0 + lane;
+                const bool kept = r < H0 && (r == 0 || ((kw[r >> 5] >> (r & 31)) & 1u));
+                const unsigned int b = __ballot_sync(0xffffffffu, kept);
+                if (kept) slot[base + __popc(b & ((1u << lane) - 1u))] = r;
+                base += __popc(b);
+            }
+            if (lane == 0) s_kept = base;
+        }
+        __syncthreads();
+        H0k = s_kept;
+    }
     // restore(): root snapshot -> shared memory, one TMA bulk copy per row (backup.ts:53-105)
-    if (tid == 0) mbar_expect_tx(&s_bar, (uint32_t)(H0 * Ws * sizeof(double)));
+    if (tid == 0) mbar_expect_tx(&s_bar, (uint32_t)(H0k * Ws * sizeof(double)));
     __syncthreads();
-    for (int r = tid; r < H0; r += NT)
-        tma_bulk_g2s(Ms + (size_t)r * Ws, nb.rootM + (size_t)r * nb.root_stride, (uint32_t)(Ws * sizeof(double)), &s_bar);
+    for (int r = tid; r < H0k; r += NT) {
+        const int src = SUBSET ? slot[r] : r;
+        tma_bulk_g2s(Ms + (size_t)r * Ws, nb.rootM + (size_t)src * nb.root_stride, (uint32_t)(Ws * sizeof(double)), &s_bar);
+    }
     // the cut list may live in mapped host memory: one PCIe round trip, overlapped with the restore
     int c0, nc;
     if (nb.n_inline > 0) { c0 = nb.cut_off_inline[node]; nc = nb.cut_off_inline[node + 1] - c0; }
@@ -157,29 +188,32 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
     const double prec = T.prec;
     int *vcol = T.vcol;
     for (int h = tid; h < nc; h += NT) cutS[h] = nb.cuts[c0 + h];
-    for (int r = tid; r < H0; r += NT) vrow[r] = __ldg(nb.root_vrow + r);
+    for (int r = tid; r < H0k; r += NT) vrow[r] = __ldg(nb.root_vrow + (SUBSET ? slot[r] : r));
     for (int c = tid; c < W; c += NT) vcol[c] = __ldg(nb.root_vcol + c);
-    for (int r = tid; r < nb.Hcap; r += NT) slot[r] = r;
-    const int Hn = H0 + nc;
+    if (!SUBSET)
+        for (int r = tid; r < nb.Hcap; r += NT) slot[r] = r;
+    const int Hn = H0k + nc;
     if (tid == 0) tl0 = globaltimer_ns() - t_start;
     mbar_wait(&s_bar, 0);
     __syncthreads();
+    if (SUBSET)  // nobody reads slot until the barrier after the cut rows
+        for (int r = tid; r < nb.Hcap; r += NT) slot[r] = r;
     if (tid == 0) tl1 = globaltimer_ns() - t_start;
     // addCutConstraints(): every cut row is expressed in the ROOT basis, so the rows are independent:
     // one warp per cut, no CTA barrier inside
     for (int h = warp; h < nc; h += NW) {
         const CutDev cut = cutS[h];
         int s_row, s_col;
-        cut_lookup(vrow, H0, vcol, W, cut.var_index, lane, 32, s_row, s_col);
+        cut_lookup(vrow, H0k, vcol, W, cut.var_index, lane, 32, s_row, s_col);
         s_row = __reduce_max_sync(0xffffffffu, s_row);
         s_col = __reduce_max_sync(0xffffffffu, s_col);
         const double *vr = s_row < 0 ? nullptr : Ms + (size_t)s_row * Ws;
-        double *cutrow = Ms + (size_t)(H0 + h) * Ws;
+        double *cutrow = Ms + (size_t)(H0k + h) * Ws;
         if (vr != nullptr)  // one loop per case: neither tests the case per entry
             for (int c = lane; c < W; c += 32) cutrow[c] = cut_entry(cut, c, s_col, vr);
         else
             for (int c = lane; c < W; c += 32) cutrow[c] = cut_entry(cut, c, s_col, nullptr);
-        if (lane == 0) vrow[H0 + h] = nb.first_index + h;
+        if (lane == 0) vrow[H0k + h] = nb.first_index + h;
     }
     __syncthreads();
     if (tid == 0) tl2 = globaltimer_ns() - t_start;
@@ -218,8 +252,12 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
                     if (v < b.v) { b.v = v; b.i = r; }
                 }
                 b = warp_reduce_vi<true>(b);
-                if (b.i == INT_MAX) phase = 2;  // feasible (simplex.ts:51-54)
-                else rstar = b.i;
+                if (b.i == INT_MAX) {  // feasible (simplex.ts:51-54)
+                    if (SUBSET && nb.phase1_only) { status = ST_P1_DONE; go = 0; }
+                    else phase = 2;
+                } else {
+                    rstar = b.i;
+                }
             }
             if (go && rstar < 0) {  // phase 2
                 if (next_c < 0) next_c = warp_price(T, cost, vcol, W, lane, &next_neg);

@@ -82,6 +82,43 @@ def mixed_lp_model(n_vars: int, n_cons: int, seed: int = 7, density: float = 0.7
             "opType": "max" if rng.random() < 0.5 else "min", "constraints": constraints, "variables": variables}
 
 
+def planted_infeasible_model(n_vars: int, n_cons: int, k: int, seed: int = 12345) -> dict:
+    """An infeasible LP whose only irreducible infeasible subset is known: k - 1 rows `x_j <= 1` and one row
+    `sum x_j >= k` over the same k - 1 variables (names `conflict*`), spread through the row order, plus a background
+    of n_cons - k random packing rows (`max`, entries U{1..20} at density 0.5) on the other n_vars - k + 1 variables,
+    each satisfied with a margin U{1..20} at an interior point x0 ~ U[0.5, 1.5].  The background is feasible and
+    shares no variable with the planted rows, so it is in no infeasible subset."""
+    assert 2 <= k <= n_cons and k - 1 < n_vars
+    rng = np.random.default_rng(seed)
+    n_bg = n_vars - (k - 1)
+    planted_vars = [f"p{j}" for j in range(k - 1)]
+    bg_vars = [f"x{j}" for j in range(n_bg)]
+    planted_pos = set(int(i) for i in rng.choice(n_cons, size=k, replace=False))
+    x0 = rng.uniform(0.5, 1.5, size=n_bg)
+    variables = {v: {"objective": float(rng.integers(1, 51))} for v in planted_vars + bg_vars}
+    constraints = {}
+    p = 0
+    for i in range(n_cons):
+        if i in planted_pos:
+            name = f"conflict{p}"
+            if p < k - 1:
+                constraints[name] = {"max": 1.0}
+                variables[planted_vars[p]][name] = 1.0
+            else:
+                constraints[name] = {"min": float(k)}
+                for v in planted_vars:
+                    variables[v][name] = 1.0
+            p += 1
+            continue
+        name = f"c{i}"
+        a = np.where(rng.random(n_bg) < 0.5, rng.integers(1, 21, size=n_bg), 0).astype(np.float64)
+        constraints[name] = {"max": float(np.ceil(a @ x0)) + float(rng.integers(1, 21))}
+        for j in np.nonzero(a)[0]:
+            variables[bg_vars[j]][name] = float(a[j])
+    return {"name": f"Planted_{n_vars}x{n_cons}_k{k}_seed{seed}", "optimize": "objective", "opType": "max",
+            "constraints": constraints, "variables": variables}
+
+
 def knapsack_mip_model(n_items: int, n_cons: int, seed: int = 12345, tolerance: float = 0.0) -> dict:
     """Multi-dimensional 0/1 knapsack (SURVEY.md 8d config 5): a_ij ~ U{1..50} dense,
     b_i = floor(0.5 * sum_j a_ij), c_j ~ U{1..50}; every binary adds an `x <= 1` row

@@ -79,6 +79,13 @@ class Solution:  # solution.ts:16-61
         from .sensitivity import report
         return report(self)
 
+    def iis(self) -> dict:
+        """An irreducible infeasible subset of the rows of this infeasible continuous LP (DESIGN.md section 2c):
+        {"constraints": [{name, type, rhs}, ...], "names": [...], "irreducible": bool, "lps": int}; raises
+        ValueError where it is not defined."""
+        from .iis import compute
+        return compute(self)
+
     def generateSolutionSet(self) -> dict:
         t = self._tableau
         out: dict = {}
@@ -580,6 +587,18 @@ class GpuTableau:
         _lib.check(self.context.lib.jslp_sensitivity(self._h(), col_lo.ctypes.data, col_hi.ctypes.data,
                                                      row_lo.ctypes.data, row_hi.ctypes.data))
         return col_lo, col_hi, row_lo, row_hi
+
+    def feasibility_batch(self, keep):
+        """jslp_feasibility_batch: phase 1 (cycle check on) of the row subsets keep[s] (n_sets x height, nonzero =
+        keep; row 0 is always kept) of the saved snapshot.  Returns (verdict, pivots) int32 arrays, verdict 0 =
+        feasible, 1 = infeasible, 2 = undecided (DESIGN.md section 2c).  Leaves the tableau equal to its snapshot."""
+        keep = np.ascontiguousarray(keep, dtype=np.uint8)
+        n = keep.shape[0]
+        verdict, pivots = np.empty(n, dtype=np.int32), np.empty(n, dtype=np.int32)
+        _lib.check(self.context.lib.jslp_feasibility_batch(self._h(), keep.ctypes.data, n, verdict.ctypes.data,
+                                                           pivots.ctypes.data))
+        self._refresh_dims()
+        return verdict, pivots
 
     def optional_reduced_costs(self) -> np.ndarray:
         return self._download("opt")
