@@ -208,6 +208,22 @@ int jslp_sensitivity(jslp_tab *tab, double *col_lo, double *col_hi, double *row_
  * phase-1 pivots.  The cycle check is always on.  On return the tableau equals its snapshot. */
 int jslp_feasibility_batch(jslp_tab *tab, const uint8_t *keep, int n_sets, int32_t *verdict, int32_t *pivots);
 
+/* Parametric path of the current (optimal) tableau: one right-hand side (kind 0) or one cost (kind 1) moves from
+ * theta0 to target, with one pivot per basis change (no reference counterpart; DESIGN.md section 2d).
+ *   labels / signs  n_labels entries: the moved slack labels (1 or 2, in tableau row order) with sign g * s_i, or the
+ *                   moved variable's label (1) with sign g * sigma; g = +1 when target >= theta0, s_i = +1 for a
+ *                   `max` row and -1 for a `min` row, sigma = +1 for maximisation and -1 for minimisation
+ *   max_breaks      at most this many pieces (>= 1); the output arrays hold max_breaks entries
+ *   per piece k < *n_breaks:  theta[k] where it ends, obj_raw[k] = M[0,0] there, dobj[k] = the direction's objective
+ *                   entry it moved along, rc_lbl[4k .. 4k+3] = pivot row, pivot column, leaving and entering label of
+ *                   the basis change that ends it (-1 where there is none)
+ *   stop            1 reached target, 2 infeasible beyond theta, 3 unbounded beyond theta, 4 max_breaks pieces
+ *   end_rhs / end_vrow  height entries: column 0 and the row labels at the end of the path
+ * The tableau, its labels, the staged pivot and the pivot record are restored before the call returns. */
+int jslp_parametric(jslp_tab *tab, int kind, const int32_t *labels, const double *signs, int n_labels,
+                    double theta0, double target, int max_breaks, double *theta, double *obj_raw, double *dobj,
+                    int32_t *rc_lbl, int *n_breaks, int *stop, double *end_rhs, int32_t *end_vrow);
+
 /* Multi-GPU communicator of the branch-and-cut frontier (one process per GPU).  NCCL is loaded at run time;
  * without libnccl these calls fail with JSLP_E_UNSUPPORTED and single-GPU use is unaffected.  Rank 0 obtains a
  * 128-byte unique id and hands it to the other ranks through whatever bootstrap the host has (the N-API host:

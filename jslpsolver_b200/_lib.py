@@ -97,6 +97,8 @@ SYMBOLS = [
     ("jslp_pivot_log", C.c_int, [P, P, C.c_int, C.POINTER(C.c_int)]),
     ("jslp_sensitivity", C.c_int, [P, P, P, P, P]),
     ("jslp_feasibility_batch", C.c_int, [P, P, C.c_int, P, P]),
+    ("jslp_parametric", C.c_int, [P, C.c_int, P, P, C.c_int, C.c_double, C.c_double, C.c_int, P, P, P, P,
+                                  C.POINTER(C.c_int), C.POINTER(C.c_int), P, P]),
     ("jslp_branch_and_cut", C.c_int, [P, C.POINTER(BnbOpts), C.POINTER(BnbStatus), P, C.c_int]),
     ("jslp_bnb_node_log", C.c_int, [P, P, C.c_int64, C.POINTER(C.c_int64)]),
     ("jslp_bnb_solution", C.c_int, [P, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_int32), P, P, C.c_int]),

@@ -169,6 +169,10 @@ struct jslp_tab {
     size_t sens_cap = 0;
     void *d_iis = nullptr;  // jslp_feasibility_batch: packed keep masks / the gathered row list
     size_t iis_bytes = 0;
+    void *d_param = nullptr, *d_plog = nullptr;  // jslp_parametric: path state and its breakpoint log
+    int param_cap = 0;
+    cudaGraphExec_t param_graph = nullptr;
+    int param_key[3] = {0, 0, 0};  // step grid, shared memory and variant the graph was captured for
 };
 
 extern "C" const char *jslp_last_error(void) { return g_err.c_str(); }
@@ -334,6 +338,8 @@ extern "C" void jslp_tab_destroy(jslp_tab *t) {
     cudaFreeHost(t->h_rec); cudaFreeHost(t->h_log); cudaFreeHost(t->h_mip); cudaFreeHost(t->h_cuts);
     cudaFree(t->d_count); cudaFreeHost(t->h_count);
     cudaFree(t->d_sens); cudaFree(t->d_iis);
+    cudaFree(t->d_param); cudaFree(t->d_plog);
+    if (t->param_graph) cudaGraphExecDestroy(t->param_graph);
     free_saved(t->saved);
     free_snap(t->snaps[0]);
     free_snap(t->snaps[1]);
@@ -1351,3 +1357,4 @@ extern "C" int jslp_pivot_log(jslp_tab *t, int32_t *entries, int cap, int *n) {
 #include "jslp_bnb.cuh"
 #include "jslp_sensitivity.cuh"
 #include "jslp_iis.cuh"
+#include "jslp_parametric.cuh"

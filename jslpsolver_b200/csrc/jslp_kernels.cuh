@@ -204,6 +204,25 @@ __device__ __forceinline__ void ratio_step(int r, double col, double rhs, bool i
     if (quo > prec && best.v > quo) { best.v = quo; best.i = r; }
 }
 
+// One candidate i of the parametric min-quotient tests (DESIGN.md section 2d): the primal step bound -M[r,0] / D[r]
+// (num = -M[r,0], den = D[r]), the dual ratio test M[0,c] / M[r*,c], and the cost step bound -M[0,c] / E[c] (num =
+// M[0,c], den = -E[c]; negating the divisor instead of the dividend gives the same IEEE quotient).  A restricted
+// candidate takes part when den < -prec, an unrestricted one offers 0 when |den| > prec; a quotient below 0 or -0
+// counts as +0 and a NaN quotient takes no part.  Lowest i on ties when candidates come in increasing order.
+template <DivFn DIV = ddiv>
+__device__ __forceinline__ void param_ratio(int i, double num, double den, bool unres, double prec, VI &best) {
+    double q;
+    if (unres) {
+        if (!(fabs(den) > prec)) return;
+        q = 0.0;
+    } else {
+        if (!(den < -prec)) return;
+        q = DIV(num, den);
+        if (!(q > 0.0) && q == q) q = 0.0;
+    }
+    if (q < best.v) { best.v = q; best.i = i; }
+}
+
 // One column of the phase-1 entering-column scan (simplex.ts:56-76): the column qualifies when its variable is
 // unrestricted or coef (the leaving row's entry) < -prec, and the largest -cost / coef wins (lowest column on ties when
 // columns come in increasing order).  cost() yields the cost-row entry; it runs for qualifying columns only.

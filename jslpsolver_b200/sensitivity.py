@@ -11,21 +11,21 @@ import math
 INF = math.inf
 
 
-def _check(solution) -> None:
+def _check(solution, what: str = "sensitivity()") -> None:
     t = solution._tableau
     m = getattr(t, "model", None)
     if m is None:
-        raise ValueError("sensitivity() needs a solution of a Model (Solve(model, full=True) or Model.solve())")
+        raise ValueError(f"{what} needs a solution of a Model (Solve(model, full=True) or Model.solve())")
     if m.getNumberOfIntegerVariables() > 0:
-        raise ValueError("sensitivity() is defined for continuous LPs only: the model has integer or binary variables")
+        raise ValueError(f"{what} is defined for continuous LPs only: the model has integer or binary variables")
     if any(c.relaxation is not None for c in m.constraints) or any(v.priority for v in m.variables):
-        raise ValueError("sensitivity() does not support soft constraints (weight / priority) or optional objectives")
+        raise ValueError(f"{what} does not support soft constraints (weight / priority) or optional objectives")
     if not solution.feasible:
-        raise ValueError("sensitivity() needs an optimal solution: the LP is infeasible")
+        raise ValueError(f"{what} needs an optimal solution: the LP is infeasible")
     if not solution.bounded:
-        raise ValueError("sensitivity() needs an optimal solution: the LP is unbounded")
+        raise ValueError(f"{what} needs an optimal solution: the LP is unbounded")
     if t.handle is None or t._solved_version != t._version or solution._version != t._version:
-        raise ValueError("sensitivity() needs the tableau as the solve of this solution left it: "
+        raise ValueError(f"{what} needs the tableau as the solve of this solution left it: "
                          "it has not been solved, or it was edited or solved again since")
 
 

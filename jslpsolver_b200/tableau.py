@@ -86,6 +86,14 @@ class Solution:  # solution.ts:16-61
         from .iis import compute
         return compute(self)
 
+    def parametric(self, constraint=None, variable=None, side=None, to=None) -> dict:
+        """The optimal result of this continuous LP as one right-hand side (constraint=name, side= for a constraint
+        with a min and a max bound) or one cost (variable=id) moves from its current value to `to`: linear pieces
+        between the basis changes, each with its slope and the basis change that ends it (DESIGN.md section 2d).
+        The tableau is left unchanged; raises ValueError where sensitivity() does and for unknown names."""
+        from .parametric import compute
+        return compute(self, constraint=constraint, variable=variable, side=side, to=to)
+
     def generateSolutionSet(self) -> dict:
         t = self._tableau
         out: dict = {}
@@ -599,6 +607,25 @@ class GpuTableau:
                                                            pivots.ctypes.data))
         self._refresh_dims()
         return verdict, pivots
+
+    def parametric_path(self, kind: int, labels, signs, theta0: float, target: float, max_breaks: int) -> dict:
+        """jslp_parametric: the breakpoint records of the path of one right-hand side (kind 0) or one cost (kind 1)
+        from theta0 to target (DESIGN.md section 2d), the stop code, and column 0 and the row labels at its end.
+        The device tableau is restored before the call returns."""
+        H = self.height
+        lab = np.ascontiguousarray(labels, dtype=np.int32)
+        sg = np.ascontiguousarray(signs, dtype=np.float64)
+        theta, obj, dobj = (np.empty(max_breaks, dtype=np.float64) for _ in range(3))
+        rc = np.empty((max_breaks, 4), dtype=np.int32)
+        end_rhs, end_vrow = np.empty(H, dtype=np.float64), np.empty(H, dtype=np.int32)
+        n, stop = C.c_int(), C.c_int()
+        _lib.check(self.context.lib.jslp_parametric(
+            self._h(), int(kind), lab.ctypes.data, sg.ctypes.data, len(lab), float(theta0), float(target),
+            int(max_breaks), theta.ctypes.data, obj.ctypes.data, dobj.ctypes.data, rc.ctypes.data, C.byref(n),
+            C.byref(stop), end_rhs.ctypes.data, end_vrow.ctypes.data))
+        k = n.value
+        return {"theta": theta[:k], "obj_raw": obj[:k], "dobj": dobj[:k], "rc_lbl": rc[:k], "stop": stop.value,
+                "end_rhs": end_rhs, "end_vrow": end_vrow}
 
     def optional_reduced_costs(self) -> np.ndarray:
         return self._download("opt")
