@@ -38,6 +38,44 @@ def dense_packing_lp_tableau(n_vars: int, n_cons: int, seed: int = 12345) -> Ini
                           np.zeros((0, W), dtype=np.float64))
 
 
+def lp_model(A, b, c, lower=None, maximize: bool = True) -> dict:
+    """A dense LP as a jsLPSolver JSON model: row i is `min: b_i` where lower[i] is set, `max: b_i` otherwise.  Every
+    entry of A except +0.0 becomes a term (so -0.0 survives as an explicit coefficient)."""
+    A, b, c = np.asarray(A, dtype=np.float64), np.asarray(b, dtype=np.float64), np.asarray(c, dtype=np.float64)
+    lower = np.zeros(len(b), dtype=bool) if lower is None else np.asarray(lower, dtype=bool)
+    present = (A != 0) | np.signbit(A) | np.isnan(A)
+    constraints = {f"c{i}": {"min" if lower[i] else "max": float(b[i])} for i in range(len(b))}
+    variables = {}
+    for j in range(A.shape[1]):
+        v = {"objective": float(c[j])}
+        for i in np.nonzero(present[:, j])[0]:
+            v[f"c{i}"] = float(A[i, j])
+        variables[f"x{j}"] = v
+    return {"name": f"LP_{A.shape[1]}x{A.shape[0]}", "optimize": "objective", "opType": "max" if maximize else "min",
+            "constraints": constraints, "variables": variables}
+
+
+def lp_tableau(A, b, c, lower=None, maximize: bool = True) -> InitialTableau:
+    """The tableau `Model.loadJson(lp_model(A, b, c, lower, maximize)).initial_tableau()` builds, emitted directly (for
+    shapes where the JSON front end is slow): a `min` row is stored negated (tableau.ts:364-378), an absent term stays
+    +0.0, and a falsy cost enters as 0 times the objective's sign."""
+    A, b, c = np.asarray(A, dtype=np.float64), np.asarray(b, dtype=np.float64), np.asarray(c, dtype=np.float64)
+    n_cons, n_vars = A.shape
+    lower = np.zeros(n_cons, dtype=bool) if lower is None else np.asarray(lower, dtype=bool)
+    present = (A != 0) | np.signbit(A) | np.isnan(A)
+    s = np.where(lower, -1.0, 1.0)
+    sign = 1.0 if maximize else -1.0
+    H, W = n_cons + 1, n_vars + 1
+    M = np.zeros((H, W), dtype=np.float64)
+    M[0, 1:] = sign * np.where((c != 0) & ~np.isnan(c), c, 0.0)
+    M[1:, 0] = s * b
+    M[1:, 1:] = np.where(present, s[:, None] * A, 0.0)
+    vrow = np.concatenate([[-1], np.arange(n_cons)]).astype(np.int32)
+    vcol = np.concatenate([[-1], n_cons + np.arange(n_vars)]).astype(np.int32)
+    return InitialTableau(M, vrow, vcol, np.zeros(W + H - 2, dtype=np.uint8), np.zeros(0, dtype=np.int32), [],
+                          np.zeros((0, W), dtype=np.float64))
+
+
 def dense_packing_lp_model(n_vars: int, n_cons: int, seed: int = 12345) -> dict:
     """Same instance as a jsLPSolver JSON model (use for moderate sizes)."""
     A, b, c = dense_packing_lp_arrays(n_vars, n_cons, seed)

@@ -78,7 +78,10 @@ def test_fixture_subsets_match_oracle(fx, path):
 
 SEEDED = {"dense 30x20": ("dense", 30, 20, 1), "mixed 40x30": ("mixed", 40, 30, 11), "mixed 90x60": ("mixed", 90, 60, 13),
           "mixed 40x30 unrestricted": ("mixed_free", 40, 30, 12), "random 40x30": ("random", 40, 30, 5),
-          "random 30x25 unrestricted": ("random_free", 30, 25, 6)}
+          "random 30x25 unrestricted": ("random_free", 30, 25, 6),
+          # root heights 32, 33, 64, 65 (cost row included): the keep mask fills one / spills into a second 32-bit word
+          "mixed 20x31": ("mixed", 20, 31, 31), "mixed 20x32": ("mixed", 20, 32, 32),
+          "mixed 24x63": ("mixed", 24, 63, 33), "mixed 24x64": ("mixed", 24, 64, 34)}
 
 
 def _seeded(kind, n, mcons, seed):

@@ -34,8 +34,9 @@ def oracle_lp(it, precision=1e-8, check_cycles=True, log=1 << 16):
     return t
 
 
-def gpu_lp(it, engine, precision=1e-8, batch=None, log=1 << 16):
-    """engine: JSLP_OPT_ENGINE value, or a tuple (engine, lookahead, step variant)."""
+def gpu_lp(it, engine, precision=1e-8, batch=None, log=1 << 16, grid_per_sm=None, timeline=None):
+    """engine: JSLP_OPT_ENGINE value, or a tuple (engine, lookahead, step variant[, PDL[, ping-pong]]).
+    grid_per_sm: JSLP_OPT_GRID_PER_SM (step CTAs per SM); timeline: JSLP_OPT_TIMELINE (pivot steps recorded)."""
     from jslpsolver_b200 import _lib
     from jslpsolver_b200.tableau import GpuTableau
     lookahead = variant = pdl = pingpong = None
@@ -58,6 +59,10 @@ def gpu_lp(it, engine, precision=1e-8, batch=None, log=1 << 16):
         g.set_option(_lib.OPT_PINGPONG, pingpong)
     if batch:
         g.set_option(_lib.OPT_BATCH, batch)
+    if grid_per_sm is not None:
+        g.set_option(_lib.OPT_GRID_PER_SM, grid_per_sm)
+    if timeline is not None:
+        g.set_option(_lib.OPT_TIMELINE, timeline)
     return g
 
 

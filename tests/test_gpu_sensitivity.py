@@ -72,7 +72,12 @@ SEEDED = {"dense 5x4": ("dense", 5, 4, 1), "dense 64x64": ("dense", 64, 64, 3), 
           "mixed 12x9": ("mixed", 12, 9, 11), "mixed 120x80": ("mixed", 120, 80, 13),
           "mixed 40x30 unrestricted": ("mixed_free", 40, 30, 12), "mixed 260x200 unrestricted": ("mixed_free", 260, 200, 14),
           "wide mixed 2100x30": ("mixed", 2100, 30, 15), "tall dense 40x10000": ("dense", 40, 10000, 8),
-          "config 3 dense 2000x2000": ("dense", 2000, 2000, 12345)}
+          "config 3 dense 2000x2000": ("dense", 2000, 2000, 12345),
+          # k_sensitivity's partition edges: one 256-column block exactly and one column past it (W = 256, 257, 512,
+          # 513), and H - 1 = 2112 / 2113 rows: 8-row warp groups x 264 row blocks end on / one row past a full pass
+          "dense 255x40": ("dense", 255, 40, 21), "mixed 256x30": ("mixed", 256, 30, 22),
+          "dense 511x24": ("dense", 511, 24, 23), "mixed 512x20": ("mixed", 512, 20, 24),
+          "tall dense 20x2112": ("dense", 20, 2112, 25), "tall dense 20x2113": ("dense", 20, 2113, 26)}
 
 
 def _seeded_tableau(kind, n, m, seed):
