@@ -224,6 +224,28 @@ int jslp_parametric(jslp_tab *tab, int kind, const int32_t *labels, const double
                     double theta0, double target, int max_breaks, double *theta, double *obj_raw, double *dobj,
                     int32_t *rc_lbl, int *n_breaks, int *stop, double *end_rhs, int32_t *end_vrow);
 
+/* One edit of a what-if scenario: kind 0 = Tableau.updateRightHandSide(index, difference) of the constraint row with
+ * slack index `index`, kind 1 = Tableau.updateCost(index, difference) of the priority-0 variable `index`
+ * (dynamic-modification.ts:78-106,137-160).  `difference` is what setRightHandSide / setCost pass.                 */
+typedef struct {
+    int32_t kind;
+    int32_t index;
+    double difference;
+} jslp_scenario_edit;
+
+/* What-if scenarios on the current (solved) tableau, DESIGN.md section 2e.  Scenario s is edits[offsets[s] ..
+ * offsets[s+1]) (every kind-0 edit before every kind-1 edit) applied in order to the current tableau, then simplex()
+ * with check_cycles; each scenario starts from the current tableau.  Per scenario:
+ *   status[s]     0 optimal, 1 infeasible, 2 unbounded, 3 cycled (the cycle check fired)
+ *   eval_raw[s]   matrix[0][0] as simplex() left it (Tableau.evaluation before rounding, when optimal)
+ *   p1[s], p2[s]  phase-1 / phase-2 pivots
+ *   rhs, vrow     height entries each at s * height: the final right-hand-side column and varIndexByRow
+ * The tableau, its labels, the staged pivot, the pivot record, the scalar Tableau state, the pivot log and the
+ * jslp_save snapshot are as they were when the call returns.  No optional objectives. */
+int jslp_scenario_batch(jslp_tab *tab, const jslp_scenario_edit *edits, const int32_t *offsets, int n_scenarios,
+                        int check_cycles, int32_t *status, double *eval_raw, int32_t *p1, int32_t *p2, double *rhs,
+                        int32_t *vrow);
+
 /* Multi-GPU communicator of the branch-and-cut frontier (one process per GPU).  NCCL is loaded at run time;
  * without libnccl these calls fail with JSLP_E_UNSUPPORTED and single-GPU use is unaffected.  Rank 0 obtains a
  * 128-byte unique id and hands it to the other ranks through whatever bootstrap the host has (the N-API host:

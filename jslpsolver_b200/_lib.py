@@ -31,6 +31,10 @@ class Cut(C.Structure):
     _fields_ = [("type", C.c_int32), ("var_index", C.c_int32), ("value", C.c_double)]
 
 
+class ScenarioEdit(C.Structure):  # jslp_scenario_edit
+    _fields_ = [("kind", C.c_int32), ("index", C.c_int32), ("difference", C.c_double)]
+
+
 ALL_GATHER_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_int64)
 
 
@@ -99,6 +103,7 @@ SYMBOLS = [
     ("jslp_feasibility_batch", C.c_int, [P, P, C.c_int, P, P]),
     ("jslp_parametric", C.c_int, [P, C.c_int, P, P, C.c_int, C.c_double, C.c_double, C.c_int, P, P, P, P,
                                   C.POINTER(C.c_int), C.POINTER(C.c_int), P, P]),
+    ("jslp_scenario_batch", C.c_int, [P, P, P, C.c_int, C.c_int, P, P, P, P, P, P]),
     ("jslp_branch_and_cut", C.c_int, [P, C.POINTER(BnbOpts), C.POINTER(BnbStatus), P, C.c_int]),
     ("jslp_bnb_node_log", C.c_int, [P, P, C.c_int64, C.POINTER(C.c_int64)]),
     ("jslp_bnb_solution", C.c_int, [P, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_int32), P, P, C.c_int]),

@@ -149,7 +149,7 @@ struct jslp_tab {
     int g_batch = 0, g_grid = 0, g_smem = 0;
     cudaEvent_t ev_slot[2] = {nullptr, nullptr};
     Saved saved;
-    Snapshot snaps[2];  // one restart point per in-flight batch
+    Snapshot snaps[3];  // one restart point per in-flight batch; [2] = jslp_scenario_batch's source tableau
     std::vector<NodeLogEntry> node_log;
     struct StoredSolution { double evaluation; std::vector<int> vrow; std::vector<double> rhs; };
     std::vector<StoredSolution> solutions;  // keep_solutions (branch-and-cut.ts:143-153)
@@ -169,6 +169,8 @@ struct jslp_tab {
     size_t sens_cap = 0;
     void *d_iis = nullptr;  // jslp_feasibility_batch: packed keep masks / the gathered row list
     size_t iis_bytes = 0;
+    void *d_scen = nullptr;  // jslp_scenario_batch: offsets, resolved edits and per-scenario outputs of one chunk
+    size_t scen_bytes = 0;
     void *d_param = nullptr, *d_plog = nullptr;  // jslp_parametric: path state and its breakpoint log
     int param_cap = 0;
     cudaGraphExec_t param_graph = nullptr;
@@ -337,12 +339,13 @@ extern "C" void jslp_tab_destroy(jslp_tab *t) {
     cudaFree(t->d_T); cudaFree(t->d_rec); cudaFree(t->d_mip); cudaFree(t->d_cuts);
     cudaFreeHost(t->h_rec); cudaFreeHost(t->h_log); cudaFreeHost(t->h_mip); cudaFreeHost(t->h_cuts);
     cudaFree(t->d_count); cudaFreeHost(t->h_count);
-    cudaFree(t->d_sens); cudaFree(t->d_iis);
+    cudaFree(t->d_sens); cudaFree(t->d_iis); cudaFree(t->d_scen);
     cudaFree(t->d_param); cudaFree(t->d_plog);
     if (t->param_graph) cudaGraphExecDestroy(t->param_graph);
     free_saved(t->saved);
     free_snap(t->snaps[0]);
     free_snap(t->snaps[1]);
+    free_snap(t->snaps[2]);
     if (t->ev_slot[0]) cudaEventDestroy(t->ev_slot[0]);
     if (t->ev_slot[1]) cudaEventDestroy(t->ev_slot[1]);
     t->rbufs.release();
@@ -815,10 +818,10 @@ static int run_lp_resident(jslp_tab *t, int check_cycles, jslp_lp_status *out, b
     nb.H0 = t->H; nb.root_stride = t->stride; nb.first_index = t->lastElementIndex;
     nb.Hcap = t->H; nb.Ws = Ws; nb.log_cap = log_cap; nb.max_pivots = log_cap - 2;
     if ((int)smem > rb.smem_set) {
-        CK(cudaFuncSetAttribute(k_node_batch<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CK(cudaFuncSetAttribute(k_node_batch<NODE_BRANCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         rb.smem_set = (int)smem;
     }
-    k_node_batch<false><<<1, NODE_THREADS, smem, s>>>(t->d_T, nb);
+    k_node_batch<NODE_BRANCH><<<1, NODE_THREADS, smem, s>>>(t->d_T, nb);
     ctx->launches += 1;
     CK(cudaGetLastError());
     CK(cudaStreamSynchronize(s));
@@ -1135,6 +1138,7 @@ static int grow_rows(jslp_tab *t, int need) {
     if (rc) return rc;
     free_snap(t->snaps[0]);
     free_snap(t->snaps[1]);
+    free_snap(t->snaps[2]);
     return JSLP_OK;  // descriptor is pushed by the caller; graphs read pointers through it
 }
 
@@ -1358,3 +1362,4 @@ extern "C" int jslp_pivot_log(jslp_tab *t, int32_t *entries, int cap, int *n) {
 #include "jslp_sensitivity.cuh"
 #include "jslp_iis.cuh"
 #include "jslp_parametric.cuh"
+#include "jslp_scenario.cuh"

@@ -390,10 +390,10 @@ static int eval_nodes_resident(jslp_tab *t, jslp_bnb::Branch *const *nodes, int 
         for (int i = 0; i <= n; i++) nb.cut_off_inline[i] = rb.h_off[i];
     }
     if ((int)smem > rb.smem_set) {
-        CK(cudaFuncSetAttribute(k_node_batch<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CK(cudaFuncSetAttribute(k_node_batch<NODE_BRANCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         rb.smem_set = (int)smem;
     }
-    k_node_batch<false><<<n, NODE_THREADS, smem, s>>>(t->d_T, nb);
+    k_node_batch<NODE_BRANCH><<<n, NODE_THREADS, smem, s>>>(t->d_T, nb);
     ctx->launches += 1;
     CK(cudaGetLastError());
     CK(cudaStreamSynchronize(s));  // inputs and outputs are mapped host memory: nothing to copy

@@ -13,10 +13,8 @@ namespace jslp {
 
 // dst[c] += alpha * src[c] (add != 0) or dst[c] -= alpha * src[c], c in [0, W)
 __global__ void __launch_bounds__(256) k_row_axpy(double *dst, const double *src, double alpha, int W, int add) {
-    for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < W; c += gridDim.x * blockDim.x) {
-        const double prod = __dmul_rn(alpha, src[c]);
-        dst[c] = add ? __dadd_rn(dst[c], prod) : __dsub_rn(dst[c], prod);
-    }
+    for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < W; c += gridDim.x * blockDim.x)
+        dst[c] = add ? edit_axpy_add(dst[c], alpha, src[c]) : edit_axpy_sub(dst[c], alpha, src[c]);
 }
 // M[r][dcol] -= alpha * M[r][scol] for r in [0, H) and for every optional-objective row
 __global__ void __launch_bounds__(256) k_col_axpy(const TabDev *Tp, int dcol, int scol, double alpha) {
@@ -24,10 +22,10 @@ __global__ void __launch_bounds__(256) k_col_axpy(const TabDev *Tp, int dcol, in
     const int n = T.H + T.nOpt;
     for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < n; r += gridDim.x * blockDim.x) {
         double *row = r < T.H ? T.M + (size_t)r * T.stride : T.opt + (size_t)(r - T.H) * T.stride;
-        row[dcol] = __dsub_rn(row[dcol], __dmul_rn(alpha, row[scol]));
+        row[dcol] = edit_axpy_sub(row[dcol], alpha, row[scol]);
     }
 }
-__global__ void k_entry_sub(double *p, double v) { *p = __dsub_rn(*p, v); }
+__global__ void k_entry_sub(double *p, double v) { *p = edit_sub(*p, v); }
 __global__ void k_entry_set(double *p, double v) { *p = v; }
 
 // addConstraint (dynamic-modification.ts:162-220): the new row, term by term in the caller's order.
@@ -338,6 +336,7 @@ static int restride(jslp_tab *t, int new_stride) {
     free_saved(t->saved);      // snapshots of the old layout are void
     free_snap(t->snaps[0]);
     free_snap(t->snaps[1]);
+    free_snap(t->snaps[2]);
     t->slots.release();
     drop_graphs(t);
     t->g_batch = 0;            // graphs bake the stride in: force a rebuild

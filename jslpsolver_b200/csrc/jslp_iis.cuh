@@ -3,7 +3,7 @@
 //
 // test(S) = the reference's phase 1 (simplex.ts:25-98) on cost row 0 plus the rows of S in their original order,
 // with the cycle check on.  Every slack is basic in the initial tableau, so dropping a constraint is dropping its row.
-// Sets whose rows fit shared memory run one CTA each in one k_node_batch<true> launch; the others (and any set that
+// Sets whose rows fit shared memory run one CTA each in one k_node_batch<NODE_SUBSET> launch; the others (and any set that
 // hits the in-kernel pivot or log cap) run one after another on the HBM path: the kept rows are gathered into the
 // tableau and the ordinary phase-1 path runs on them.
 #pragma once
@@ -63,7 +63,7 @@ static int feasibility_hbm(jslp_tab *t, const uint8_t *keep, int32_t *verdict, i
     return JSLP_OK;
 }
 
-// All sets in one k_node_batch<true> launch.  Sets whose log shows a cycle are undecided, stopped before the pivot
+// All sets in one k_node_batch<NODE_SUBSET> launch.  Sets whose log shows a cycle are undecided, stopped before the pivot
 // that completes the repeat, as the reference's phase 1 stops; sets that hit the pivot or log cap first go to redo.
 static int feasibility_resident(jslp_tab *t, const uint8_t *keep, int n_sets, int32_t *verdict, int32_t *pivots,
                                 std::vector<int> &redo) {
@@ -94,8 +94,8 @@ static int feasibility_resident(jslp_tab *t, const uint8_t *keep, int n_sets, in
     nb.Hcap = H0; nb.Ws = Ws; nb.log_cap = log_cap; nb.max_pivots = 100000;
     nb.keep = (const uint32_t *)t->d_iis; nb.keep_words = words; nb.phase1_only = 1;
     if (n_sets <= NODE_INLINE_OFF) nb.n_inline = n_sets;  // cut_off_inline: all zero
-    CK(cudaFuncSetAttribute(k_node_batch<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k_node_batch<true><<<n_sets, NODE_THREADS, smem, s>>>(t->d_T, nb);
+    CK(cudaFuncSetAttribute(k_node_batch<NODE_SUBSET>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k_node_batch<NODE_SUBSET><<<n_sets, NODE_THREADS, smem, s>>>(t->d_T, nb);
     ctx->launches += 1;
     CK(cudaGetLastError());
     CK(cudaStreamSynchronize(s));

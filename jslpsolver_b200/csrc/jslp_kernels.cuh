@@ -223,6 +223,13 @@ __device__ __forceinline__ void param_ratio(int i, double num, double den, bool 
     if (q < best.v) { best.v = q; best.i = i; }
 }
 
+// The dynamic-modification edits (dynamic-modification.ts:78-160), each one entry: x - d * y and x + d * y (difference
+// times entry, then subtract / add: two roundings), and x - d.  updateRightHandSide and updateCost are built from these
+// three, on the HBM tableau (jslp_dynamic.cuh) and in the scenario prologue of k_node_batch alike.
+__device__ __forceinline__ double edit_axpy_sub(double x, double d, double y) { return __dsub_rn(x, __dmul_rn(d, y)); }
+__device__ __forceinline__ double edit_axpy_add(double x, double d, double y) { return __dadd_rn(x, __dmul_rn(d, y)); }
+__device__ __forceinline__ double edit_sub(double x, double d) { return __dsub_rn(x, d); }
+
 // One column of the phase-1 entering-column scan (simplex.ts:56-76): the column qualifies when its variable is
 // unrestricted or coef (the leaving row's entry) < -prec, and the largest -cost / coef wins (lowest column on ties when
 // columns come in increasing order).  cost() yields the cost-row entry; it runs for qualifying columns only.

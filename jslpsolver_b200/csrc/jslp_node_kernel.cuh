@@ -38,22 +38,49 @@ struct NodeOut {
 };
 
 constexpr int NODE_INLINE_OFF = 64;
+
+// Launch modes of k_node_batch (a template parameter: each mode's instantiation carries only its own prologue)
+enum NodeMode : int {
+    NODE_BRANCH = 0,    // branch-and-cut nodes and engine 4: every root row, then the node's cuts
+    NODE_SUBSET = 1,    // one row subset of the root per CTA (jslp_feasibility_batch)
+    NODE_SCENARIO = 2,  // one list of right-hand-side / cost edits of the root per CTA (jslp_scenario_batch)
+};
+
+// One resolved scenario edit (DESIGN.md 2e): where updateRightHandSide / updateCost (dynamic-modification.ts:78-160)
+// write on the root tableau, and the difference.
+enum EditKind : int {
+    EDIT_RHS_COL = 0,   // slack non-basic in column pos: M[r,0] -= d * M[r,pos] for every row, row 0 included
+    EDIT_RHS_ROW = 1,   // slack basic in row pos: M[pos,0] -= d
+    EDIT_COST_ROW = 2,  // variable basic in row pos: M[0,c] += d * M[pos,c] for every column, column 0 included
+    EDIT_COST_COL = 3,  // variable non-basic in column pos: M[0,pos] -= d
+};
+struct EditDev {
+    int kind, pos;
+    double d;
+};
+
 struct NodeBatchDev {
     const double *rootM;   // root snapshot, row stride = root_stride
     const int *root_vrow, *root_vcol;
     const CutDev *cuts;    // all cuts of the batch, node n owns [cut_off[n], cut_off[n+1]); may be mapped host memory
-    const int *cut_off;
+    const int *cut_off;    // (NODE_SCENARIO: the same offsets into edits)
     NodeOut *out;          // one record per node; may be mapped host memory
     int4 *logs;            // log_cap entries per node (device memory)
     double *wb_M;          // optional write-back of node 0's final tableau (stride = root_stride)
     int *wb_vrow, *wb_vcol;
     int H0, root_stride, first_index, Hcap, Ws, log_cap, max_pivots;
-    // row-subset launches (k_node_batch<true>, jslp_feasibility_batch): node n keeps the root rows whose bits are set
+    // row-subset launches (NODE_SUBSET, jslp_feasibility_batch): node n keeps the root rows whose bits are set
     // in keep[n * keep_words ...] (device memory; row 0 is always kept), and with phase1_only the CTA stops with
-    // ST_P1_DONE where phase 1 finds no leaving row.  Not read by k_node_batch<false>.
+    // ST_P1_DONE where phase 1 finds no leaving row.  Not read by the other modes.
     const uint32_t *keep;
     int keep_words, phase1_only;
-    int n_inline;          // > 0: cut_off_inline holds the n_inline + 1 offsets (saves a PCIe round trip)
+    // scenario launches (NODE_SCENARIO, jslp_scenario_batch): node n applies edits[cut_off[n] .. cut_off[n+1]) (device
+    // memory; every right-hand-side edit before every cost edit) to the restored root, solves, and writes its final
+    // column 0 and row labels to out_rhs / out_vrow + n * H0.  Not read by the other modes.
+    const EditDev *edits;
+    double *out_rhs;
+    int *out_vrow;
+    int n_inline;         // > 0: cut_off_inline holds the n_inline + 1 offsets (saves a PCIe round trip)
     int cut_off_inline[NODE_INLINE_OFF + 1];
 };
 
@@ -112,12 +139,14 @@ struct NodePart {    // per-warp partial results of a scan
     int i[8], d[8], n[8];
 };
 
-// SUBSET = false: branch-and-cut nodes and engine 4 (every root row, then the node's cuts).  SUBSET = true: one row
+// MODE = NODE_BRANCH: branch-and-cut nodes and engine 4 (every root row, then the node's cuts).  NODE_SUBSET: one row
 // subset of the root per CTA (NodeBatchDev.keep), compacted in row order; row labels stay the root's, so the
-// unrestricted lookup and the pivot log read as on the whole tableau.  A template parameter, so that the node path
-// carries none of the subset code.
-template <bool SUBSET>
+// unrestricted lookup and the pivot log read as on the whole tableau.  NODE_SCENARIO: every root row, then the CTA's
+// edit list applied to column 0 and row 0 (DESIGN.md 2e) in place of cut rows.  A template parameter, so that the node
+// path carries none of the subset or scenario code.
+template <int MODE>
 __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, const __grid_constant__ NodeBatchDev nb) {
+    constexpr bool SUBSET = MODE == NODE_SUBSET, SCENARIO = MODE == NODE_SCENARIO;
     extern __shared__ __align__(16) unsigned char smraw[];
     __shared__ TabDev T;
     __shared__ SelSmem sel;
@@ -187,21 +216,47 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
     const int W = T.W;
     const double prec = T.prec;
     int *vcol = T.vcol;
-    for (int h = tid; h < nc; h += NT) cutS[h] = nb.cuts[c0 + h];
+    for (int h = tid; !SCENARIO && h < nc; h += NT) cutS[h] = nb.cuts[c0 + h];
     for (int r = tid; r < H0k; r += NT) vrow[r] = __ldg(nb.root_vrow + (SUBSET ? slot[r] : r));
     for (int c = tid; c < W; c += NT) vcol[c] = __ldg(nb.root_vcol + c);
     if (!SUBSET)
         for (int r = tid; r < nb.Hcap; r += NT) slot[r] = r;
-    const int Hn = H0k + nc;
+    const int Hn = SCENARIO ? H0k : H0k + nc;
     if (tid == 0) tl0 = globaltimer_ns() - t_start;
     mbar_wait(&s_bar, 0);
     __syncthreads();
     if (SUBSET)  // nobody reads slot until the barrier after the cut rows
         for (int r = tid; r < nb.Hcap; r += NT) slot[r] = r;
     if (tid == 0) tl1 = globaltimer_ns() - t_start;
+    if constexpr (SCENARIO) {
+        // setRightHandSide / setCost on the restored root (DESIGN.md 2e): every edit writes column 0 or row 0 only and
+        // reads columns >= 1 / rows >= 1, so the right-hand-side edits run as one pass over rows (each thread applies
+        // all of them to its M[r,0] in order) and the cost edits, after them, as one pass over columns.
+        const EditDev *ed = nb.edits + c0;
+        for (int r = tid; r < Hn; r += NT) {
+            double *row = Ms + (size_t)r * Ws;
+            double x = row[0];
+            for (int k = 0; k < nc; k++) {
+                const EditDev e = ed[k];
+                if (e.kind == EDIT_RHS_COL) x = edit_axpy_sub(x, e.d, row[e.pos]);
+                else if (e.kind == EDIT_RHS_ROW && e.pos == r) x = edit_sub(x, e.d);
+            }
+            row[0] = x;
+        }
+        __syncthreads();
+        for (int c = tid; c < W; c += NT) {
+            double x = Ms[c];
+            for (int k = 0; k < nc; k++) {
+                const EditDev e = ed[k];
+                if (e.kind == EDIT_COST_ROW) x = edit_axpy_add(x, e.d, Ms[(size_t)e.pos * Ws + c]);
+                else if (e.kind == EDIT_COST_COL && e.pos == c) x = edit_sub(x, e.d);
+            }
+            Ms[c] = x;
+        }
+    }
     // addCutConstraints(): every cut row is expressed in the ROOT basis, so the rows are independent:
-    // one warp per cut, no CTA barrier inside
-    for (int h = warp; h < nc; h += NW) {
+    // one warp per cut, no CTA barrier inside (a scenario's nc counts edits)
+    for (int h = warp; !SCENARIO && h < nc; h += NW) {
         const CutDev cut = cutS[h];
         int s_row, s_col;
         cut_lookup(vrow, H0k, vcol, W, cut.var_index, lane, 32, s_row, s_col);
@@ -429,6 +484,11 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
     // isIntegral / most fractional variable over the final RHS column
     for (int r = tid; r < Hn; r += NT) rhs[r] = Ms[(size_t)slot[r] * Ws];
     __syncthreads();
+    if constexpr (SCENARIO)
+        for (int r = tid; r < Hn; r += NT) {
+            nb.out_rhs[(size_t)node * H0 + r] = rhs[r];
+            nb.out_vrow[(size_t)node * H0 + r] = vrow[r];
+        }
     if (T.intpos != nullptr) {
         if (tid == 0) { T.M = rhs; T.stride = 1; T.vrow = vrow; T.H = Hn; }
         __syncthreads();

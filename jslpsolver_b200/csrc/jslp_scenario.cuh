@@ -1,0 +1,183 @@
+// jslpsolver_b200/csrc/jslp_scenario.cuh -- what-if scenarios on a solved tableau (included by jslp_api.cu after
+// jslp_parametric.cuh).  The reference re-optimises one edit at a time (Constraint.setRightHandSide / Model.setCost,
+// then simplex(); model.ts:247-273, dynamic-modification.ts:78-160); this runs a whole list of such edit sets, each
+// from the same tableau (DESIGN.md 2e).
+//
+// Every edit in scope writes column 0 or row 0 only, so one scenario is the restored tableau plus two passes.
+// Scenarios whose tableau fits shared memory run one CTA each in k_node_batch<NODE_SCENARIO>; the others, and any
+// scenario whose log shows a cycle or that hits the in-kernel pivot or log cap, run one after another on the
+// single-tableau path: restore, jslp_update_rhs / jslp_update_cost, run_lp -- the sequential definition itself.
+// The source of both is a private snapshot (snaps[2]): not the user's jslp_save snapshot, and not snaps[0..1], which
+// run_lp uses for its cycle replays.
+#pragma once
+
+enum { SCEN_OPTIMAL = 0, SCEN_INFEASIBLE = 1, SCEN_UNBOUNDED = 2, SCEN_CYCLED = 3 };
+
+static int scen_scratch(jslp_tab *t, size_t bytes) {
+    if (bytes <= t->scen_bytes) return JSLP_OK;
+    cudaFree(t->d_scen);
+    t->d_scen = nullptr;
+    t->scen_bytes = 0;
+    CK(cudaMalloc(&t->d_scen, bytes));
+    t->scen_bytes = bytes;
+    return JSLP_OK;
+}
+
+// One scenario on the single-tableau path, from the private snapshot.
+static int scenario_sequential(jslp_tab *t, const jslp_scenario_edit *e, int n, int check_cycles, int32_t *status,
+                               double *eval_raw, int32_t *p1, int32_t *p2, double *rhs, int32_t *vrow) {
+    cudaStream_t s = t->ctx->stream;
+    int rc = snapshot_copy(t, 2, false);
+    for (int k = 0; k < n && rc == JSLP_OK; k++)
+        rc = e[k].kind == 0 ? jslp_update_rhs(t, e[k].index, e[k].difference)
+                            : jslp_update_cost(t, e[k].index, -1, e[k].difference);
+    if (rc) return rc;
+    jslp_lp_status st;
+    rc = run_lp(t, 0, check_cycles, &st, false);
+    if (rc) return rc;
+    *status = st.cycled ? SCEN_CYCLED : !st.feasible ? SCEN_INFEASIBLE : !st.bounded ? SCEN_UNBOUNDED : SCEN_OPTIMAL;
+    *eval_raw = st.evaluation_raw;
+    *p1 = st.phase1_pivots;
+    *p2 = st.phase2_pivots;
+    CK(cudaMemcpy2DAsync(rhs, sizeof(double), t->hd.M, sizeof(double) * t->stride, sizeof(double), t->H,
+                         cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(vrow, t->hd.vrow, sizeof(int) * (size_t)t->H, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    return JSLP_OK;
+}
+
+// Scenarios [s0, s0 + n) in one k_node_batch<NODE_SCENARIO> launch.  Those whose log shows a cycle (per-phase
+// histories, as eval_nodes_resident) or that hit the pivot or log cap go to redo.
+static int scenario_resident(jslp_tab *t, const std::vector<EditDev> &res, const int32_t *offsets, int s0, int n,
+                             int check_cycles, int32_t *status, double *eval_raw, int32_t *p1, int32_t *p2,
+                             double *rhs, int32_t *vrow, std::vector<int> &redo) {
+    jslp_ctx *ctx = t->ctx;
+    cudaStream_t s = ctx->stream;
+    ResidentBufs &rb = t->rbufs;
+    const int H0 = t->H;
+    int Ws = 0;
+    const size_t smem = node_smem_bytes(H0, t->W, &Ws);
+    const int log_cap = t->node_log_cap;
+    int rc = rb.ensure(n, 0, log_cap);
+    if (rc) return rc;
+    // one device block per chunk: offsets, edits, final columns, final labels
+    const int e0 = offsets[s0], ne = offsets[s0 + n] - e0;
+    const size_t b_off = 0, b_ed = (sizeof(int) * (size_t)(n + 1) + 15) & ~(size_t)15;
+    const size_t b_rhs = b_ed + sizeof(EditDev) * (size_t)ne;
+    const size_t b_vrow = b_rhs + sizeof(double) * (size_t)n * H0;
+    rc = scen_scratch(t, b_vrow + sizeof(int) * (size_t)n * H0);
+    if (rc) return rc;
+    char *base = (char *)t->d_scen;
+    std::vector<int> off((size_t)n + 1);
+    for (int i = 0; i <= n; i++) off[i] = offsets[s0 + i] - e0;
+    CK(cudaMemcpyAsync(base + b_off, off.data(), sizeof(int) * (size_t)(n + 1), cudaMemcpyHostToDevice, s));
+    if (ne > 0) CK(cudaMemcpyAsync(base + b_ed, res.data() + e0, sizeof(EditDev) * (size_t)ne, cudaMemcpyHostToDevice, s));
+    NodeBatchDev nb;
+    memset(&nb, 0, sizeof(nb));
+    const Snapshot &src = t->snaps[2];
+    nb.rootM = src.M; nb.root_vrow = src.vrow; nb.root_vcol = src.vcol;
+    nb.cut_off = (const int *)(base + b_off); nb.out = rb.dv_out; nb.logs = rb.d_logs;
+    nb.H0 = H0; nb.root_stride = t->stride; nb.first_index = t->lastElementIndex;
+    nb.Hcap = H0; nb.Ws = Ws; nb.log_cap = log_cap; nb.max_pivots = 100000;
+    nb.edits = (const EditDev *)(base + b_ed);
+    nb.out_rhs = (double *)(base + b_rhs); nb.out_vrow = (int *)(base + b_vrow);
+    if (n <= NODE_INLINE_OFF) {
+        nb.n_inline = n;
+        for (int i = 0; i <= n; i++) nb.cut_off_inline[i] = off[i];
+    }
+    CK(cudaFuncSetAttribute(k_node_batch<NODE_SCENARIO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k_node_batch<NODE_SCENARIO><<<n, NODE_THREADS, smem, s>>>(t->d_T, nb);
+    ctx->launches += 1;
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(rhs + (size_t)s0 * H0, nb.out_rhs, sizeof(double) * (size_t)n * H0, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(vrow + (size_t)s0 * H0, nb.out_vrow, sizeof(int) * (size_t)n * H0, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    bool need_full = false;
+    for (int i = 0; i < n; i++) need_full |= check_cycles && !rb.h_out[i].r.overflow && rb.h_out[i].r.log_n > NODE_LOG_HEAD;
+    if (need_full) {
+        CK(cudaMemcpyAsync(rb.h_logs, rb.d_logs, sizeof(int4) * (size_t)n * log_cap, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+    }
+    for (int i = 0; i < n; i++) {
+        const NodeResult &r = rb.h_out[i].r;
+        bool again = r.overflow != 0;
+        if (!again && check_cycles) {
+            CycleHist h[2];  // (leaving, entering) per phase (simplex.ts:27,102)
+            int cs, cl;
+            const int4 *lg = r.log_n > NODE_LOG_HEAD ? rb.h_logs + (size_t)i * log_cap : rb.h_out[i].log_head;
+            for (int k = 0; k < r.log_n && k < log_cap && !again; k++)
+                again = h[((lg[k].x >> 30) & 1) ? 1 : 0].push_and_check(((long long)lg[k].z << 32) | (unsigned int)lg[k].w, &cs, &cl);
+        }
+        if (again) { redo.push_back(s0 + i); continue; }
+        status[s0 + i] = r.status == ST_OPTIMAL ? SCEN_OPTIMAL : r.status == ST_UNBOUNDED ? SCEN_UNBOUNDED : SCEN_INFEASIBLE;
+        eval_raw[s0 + i] = r.eval_raw;
+        p1[s0 + i] = r.p1;
+        p2[s0 + i] = r.p2;
+    }
+    return JSLP_OK;
+}
+
+extern "C" int jslp_scenario_batch(jslp_tab *t, const jslp_scenario_edit *edits, const int32_t *offsets, int n_scenarios,
+                                   int check_cycles, int32_t *status, double *eval_raw, int32_t *p1, int32_t *p2,
+                                   double *rhs, int32_t *vrow) {
+    if (!t) return fail(JSLP_E_INVALID, "tab is NULL");
+    if (n_scenarios < 0 || (n_scenarios > 0 && (!offsets || !status || !eval_raw || !p1 || !p2 || !rhs || !vrow)))
+        return fail(JSLP_E_INVALID, "scenario_batch: bad offsets / output arguments");
+    if (t->nOpt > 0) return fail(JSLP_E_UNSUPPORTED, "scenario_batch: optional objectives are not supported");
+    if (n_scenarios == 0) return JSLP_OK;
+    if (offsets[0] != 0) return fail(JSLP_E_INVALID, "scenario_batch: offsets[0] must be 0");
+    for (int i = 0; i < n_scenarios; i++)
+        if (offsets[i + 1] < offsets[i]) return fail(JSLP_E_INVALID, "scenario_batch: offsets must not decrease");
+    const int n_edits = offsets[n_scenarios];
+    if (n_edits > 0 && !edits) return fail(JSLP_E_INVALID, "scenario_batch: edits is NULL");
+    CK(cudaSetDevice(t->ctx->device));
+    // updateRightHandSide / updateCost resolved once against the labels: no edit pivots, so the positions are the
+    // same for every scenario and every edit of it
+    HostMaps m;
+    int rc = load_maps(t, m);
+    if (rc) return rc;
+    std::vector<EditDev> res((size_t)n_edits);
+    for (int i = 0; i < n_scenarios; i++)
+        for (int k = offsets[i]; k < offsets[i + 1]; k++) {
+            const jslp_scenario_edit &e = edits[k];
+            if (e.kind != 0 && e.kind != 1) return fail(JSLP_E_INVALID, "scenario_batch: edit kind must be 0 (rhs) or 1 (cost)");
+            if (e.kind == 0 && k > offsets[i] && edits[k - 1].kind == 1)
+                return fail(JSLP_E_INVALID, "scenario_batch: a scenario's right-hand-side edits come before its cost edits");
+            const int row = m.row_of(e.index), col = row < 0 ? m.col_of(e.index) : -1;
+            if (row < 0 && col < 0) return fail(JSLP_E_INVALID, "scenario_batch: unknown constraint or variable index");
+            if (e.kind == 0) res[k] = row < 0 ? EditDev{EDIT_RHS_COL, col, e.difference} : EditDev{EDIT_RHS_ROW, row, e.difference};
+            else res[k] = row < 0 ? EditDev{EDIT_COST_COL, col, e.difference} : EditDev{EDIT_COST_ROW, row, e.difference};
+        }
+    // the scalar Tableau state and the executed-pivot log describe the caller's tableau, not these scenarios
+    const int feasible = t->feasible, bounded = t->bounded, iters = t->simplexIters, unb = t->unboundedVar;
+    const double evaluation = t->evaluation, best = t->bestPossibleEval;
+    const size_t log_size = t->host_log.size();
+    rc = ensure_snapshot(t, 2);
+    if (rc) return rc;
+    rc = snapshot_copy(t, 2, true);
+    if (rc) return rc;
+    std::vector<int> redo;
+    if (t->engine != 1 && t->engine != 2 && resident_fits(t, t->H)) {
+        // chunks keep the per-scenario outputs on the device bounded (about 32 MB)
+        const int chunk = (int)std::max<size_t>(1, std::min<size_t>(4096, ((size_t)32 << 20) / ((size_t)12 * t->H)));
+        for (int s0 = 0; s0 < n_scenarios && rc == JSLP_OK; s0 += chunk)
+            rc = scenario_resident(t, res, offsets, s0, std::min(chunk, n_scenarios - s0), check_cycles, status, eval_raw,
+                                   p1, p2, rhs, vrow, redo);
+    } else {
+        for (int i = 0; i < n_scenarios; i++) redo.push_back(i);
+    }
+    const int H = t->H;
+    for (size_t k = 0; k < redo.size() && rc == JSLP_OK; k++) {
+        const int i = redo[k];
+        rc = scenario_sequential(t, edits + offsets[i], offsets[i + 1] - offsets[i], check_cycles, status + i,
+                                 eval_raw + i, p1 + i, p2 + i, rhs + (size_t)i * H, vrow + (size_t)i * H);
+    }
+    // the caller's tableau, labels, staged pivot and record exactly as they were
+    const int rc2 = snapshot_copy(t, 2, false);
+    if (rc == JSLP_OK) rc = rc2;
+    CK(cudaStreamSynchronize(t->ctx->stream));
+    t->feasible = feasible; t->bounded = bounded; t->simplexIters = iters; t->unboundedVar = unb;
+    t->evaluation = evaluation; t->bestPossibleEval = best;
+    if (t->host_log.size() > log_size) t->host_log.resize(log_size);
+    return rc;
+}

@@ -16,29 +16,41 @@ from .sensitivity import _check
 STOPS = {1: "reached", 2: "infeasible", 3: "unbounded", 4: "limit"}
 
 
-def _constraint_rows(m, name, side):
-    """(labels in tableau order, their row signs s_i, the side reported, the current value) of `name`."""
+def _constraint_rows(m, name, side, what="parametric()", pick="pass side='min' or side='max'"):
+    """(labels in tableau order, their row signs s_i, the side reported, the current value) of `name`.  `what` and
+    `pick` word the errors for the caller (its name, and how it chooses one bound of a min+max constraint)."""
     rows = [c for c in m.constraints if (c.name if c.name is not None else c.index) == name]
     if not rows:
-        raise ValueError(f"parametric(): no constraint named {name!r}")
+        raise ValueError(f"{what}: no constraint named {name!r}")
     if side not in (None, "min", "max", "equal"):
-        raise ValueError(f"parametric(): side must be 'min', 'max' or 'equal', not {side!r}")
+        raise ValueError(f"{what}: side must be 'min', 'max' or 'equal', not {side!r}")
     if len(rows) == 2:
         both_equal = rows[0].rhs == rows[1].rhs
         if side in ("min", "max"):
             rows = [c for c in rows if c.isUpperBound == (side == "max")]
         elif side == "equal" or both_equal:
             if not both_equal:
-                raise ValueError(f"parametric(): constraint {name!r} is not an equality; pass side='min' or side='max'")
+                raise ValueError(f"{what}: constraint {name!r} is not an equality; {pick}")
             side = "equal"
         else:
-            raise ValueError(f"parametric(): constraint {name!r} has a min and a max bound; pass side='min' or side='max'")
+            raise ValueError(f"{what}: constraint {name!r} has a min and a max bound; {pick}")
     else:
         kind = "max" if rows[0].isUpperBound else "min"
         if side not in (None, kind):
-            raise ValueError(f"parametric(): constraint {name!r} has only a {kind!r} bound")
+            raise ValueError(f"{what}: constraint {name!r} has only a {kind!r} bound")
         side = kind
     return [c.index for c in rows], [1.0 if c.isUpperBound else -1.0 for c in rows], side, float(rows[0].rhs)
+
+
+def _free_variable(m, variable, what="parametric()"):
+    """The Variable with id `variable`; presolve must not have fixed it (that zeroes its cost, section 2b)."""
+    var = next((v for v in m.variables if v.id == variable), None)
+    if var is None:
+        raise ValueError(f"{what}: no variable named {variable!r}")
+    fixed = m.presolveResult.fixedVariables if m.presolveResult is not None else {}
+    if var in fixed:
+        raise ValueError(f"{what}: presolve fixed {variable!r} and zeroed its cost, so the LP has no cost to move")
+    return var
 
 
 def compute(solution, constraint=None, variable=None, side=None, to=None, max_breaks=None) -> dict:
@@ -57,12 +69,7 @@ def compute(solution, constraint=None, variable=None, side=None, to=None, max_br
     else:
         if side is not None:
             raise ValueError("parametric(): side applies to constraints only")
-        var = next((v for v in m.variables if v.id == variable), None)
-        if var is None:
-            raise ValueError(f"parametric(): no variable named {variable!r}")
-        fixed = m.presolveResult.fixedVariables if m.presolveResult is not None else {}
-        if var in fixed:
-            raise ValueError(f"parametric(): presolve fixed {variable!r} and zeroed its cost, so the LP has no cost to move")
+        var = _free_variable(m, variable)
         labels, s, start = [var.index], [sigma], float(var.cost)
         kind, name = 1, variable
     target = float(to)

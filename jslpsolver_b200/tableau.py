@@ -20,7 +20,7 @@ from typing import Optional
 import numpy as np
 
 from . import _lib
-from ._lib import BnbOpts, BnbStatus, Cut, JslpError, LpStatus
+from ._lib import BnbOpts, BnbStatus, Cut, JslpError, LpStatus, ScenarioEdit
 
 EPSILON = 2.220446049250313e-16
 
@@ -66,6 +66,19 @@ def js_round(x: float) -> float:
     return float(f + 1) if x - f >= 0.5 else float(f)
 
 
+def solution_set(rhs, vrow, precision: float, variablesPerIndex: dict) -> dict:
+    """generateSolutionSet (solution.ts:35-60) over a right-hand-side column and its row labels: every structural
+    variable that is basic, rounded to the model precision."""
+    out: dict = {}
+    rounding = js_round(1 / precision)
+    for r in range(1, len(vrow)):
+        var = variablesPerIndex.get(int(vrow[r]))
+        if var is None or var.isSlack:
+            continue
+        out[var.id] = js_round((EPSILON + float(rhs[r])) * rounding) / rounding
+    return out
+
+
 class Solution:  # solution.ts:16-61
     def __init__(self, tableau: "GpuTableau", evaluation: float, feasible: bool, bounded: bool):
         self.feasible, self.evaluation, self.bounded = feasible, evaluation, bounded
@@ -94,20 +107,20 @@ class Solution:  # solution.ts:16-61
         from .parametric import compute
         return compute(self, constraint=constraint, variable=variable, side=side, to=to)
 
+    def scenarios(self, cases) -> list:
+        """What-if re-optimisation of this continuous LP: for each case {"rhs": {constraint: value, ...}, "cost":
+        {variable: value, ...}}, the Solve() result of the model with those right-hand sides and costs, as
+        Constraint.setRightHandSide / Model.setCost followed by a re-solve from this optimum would return it (DESIGN.md
+        section 2e).  A constraint with a min and a max bound takes {"min": a, "max": b}.  The tableau and the model are
+        left unchanged; raises ValueError where sensitivity() does, for unknown names and for bad values."""
+        from .scenarios import compute
+        return compute(self, cases)
+
     def generateSolutionSet(self) -> dict:
         t = self._tableau
-        out: dict = {}
         if t.handle is None:
-            return out
-        rhs, vrow = t.rhs_column(), t.varIndexByRow
-        rounding = js_round(1 / t.precision)
-        vpi = t.variablesPerIndex
-        for r in range(1, t.height):
-            var = vpi.get(int(vrow[r]))
-            if var is None or var.isSlack:
-                continue
-            out[var.id] = js_round((EPSILON + float(rhs[r])) * rounding) / rounding
-        return out
+            return {}
+        return solution_set(t.rhs_column(), t.varIndexByRow, t.precision, t.variablesPerIndex)
 
 
 class MilpSolution(Solution):  # solution.ts:66-80
@@ -626,6 +639,26 @@ class GpuTableau:
         k = n.value
         return {"theta": theta[:k], "obj_raw": obj[:k], "dobj": dobj[:k], "rc_lbl": rc[:k], "stop": stop.value,
                 "end_rhs": end_rhs, "end_vrow": end_vrow}
+
+    def scenario_batch(self, edits, offsets, check_cycles: Optional[bool] = None) -> dict:
+        """jslp_scenario_batch: edits = [(kind, index, difference), ...] with kind 0 = updateRightHandSide and 1 =
+        updateCost; scenario s = edits[offsets[s]:offsets[s + 1]] applied to the current tableau, then simplex() (the
+        model's cycle check unless check_cycles is given), each from the current tableau (DESIGN.md section 2e).
+        Returns the per-scenario status (0 optimal, 1 infeasible, 2 unbounded, 3 cycled), raw evaluation, phase-1 /
+        phase-2 pivots, and the final right-hand-side column and row labels (n x height).  The tableau is unchanged."""
+        n, H = len(offsets) - 1, self.height
+        arr = (ScenarioEdit * max(1, len(edits)))()
+        for i, (kind, index, difference) in enumerate(edits):
+            arr[i].kind, arr[i].index, arr[i].difference = int(kind), int(index), float(difference)
+        off = np.ascontiguousarray(offsets, dtype=np.int32)
+        status, p1, p2 = (np.empty(n, dtype=np.int32) for _ in range(3))
+        eval_raw = np.empty(n, dtype=np.float64)
+        rhs, vrow = np.empty((n, H), dtype=np.float64), np.empty((n, H), dtype=np.int32)
+        cc = self._check_cycles() if check_cycles is None else int(bool(check_cycles))
+        _lib.check(self.context.lib.jslp_scenario_batch(
+            self._h(), arr, off.ctypes.data, n, cc, status.ctypes.data, eval_raw.ctypes.data, p1.ctypes.data,
+            p2.ctypes.data, rhs.ctypes.data, vrow.ctypes.data))
+        return {"status": status, "eval_raw": eval_raw, "p1": p1, "p2": p2, "rhs": rhs, "vrow": vrow}
 
     def optional_reduced_costs(self) -> np.ndarray:
         return self._download("opt")
