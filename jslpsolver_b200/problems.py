@@ -179,6 +179,28 @@ def knapsack_mip_model(n_items: int, n_cons: int, seed: int = 12345, tolerance: 
     return m
 
 
+def half_tie_mip_model(n_ints: int, group: int = 8, seed: int = 12345) -> dict:
+    """A MIP whose LP relaxation keeps many basic integer variables at exactly k + 1/2: integer x_i with a row
+    2 x_i <= 2 u_i + 1 (u_i ~ U{0..3}) and cost c_i ~ U{1..9} (max), coupled by packing rows over consecutive groups of
+    `group` variables.  Every other packing row allows sum (u_i + 1/2) over its group; the others allow 1/2 less, so
+    one variable of the group stays integral.  Whichever variable branch-and-cut branches on, the other fractions
+    stay 1/2, and the choice is decided by the position tie-break of getMostFractionalVar at nearly every node.
+    Root tableau: (n_ints + ceil(n_ints / group) + 1) x (n_ints + 1)."""
+    rng = np.random.default_rng(seed)
+    u = rng.integers(0, 4, size=n_ints)
+    c = rng.integers(1, 10, size=n_ints)
+    variables = {f"x{i}": {"value": float(c[i]), f"half{i}": 2.0} for i in range(n_ints)}
+    constraints = {f"half{i}": {"max": float(2 * u[i] + 1)} for i in range(n_ints)}
+    for g, g0 in enumerate(range(0, n_ints, group)):
+        members = range(g0, min(n_ints, g0 + group))
+        cap = float(sum(u[i] for i in members)) + 0.5 * len(members) - (0.5 if g % 2 else 0.0)
+        constraints[f"pack{g}"] = {"max": cap}
+        for i in members:
+            variables[f"x{i}"][f"pack{g}"] = 1.0
+    return {"name": f"HalfTieMIP_{n_ints}_seed{seed}", "optimize": "value", "opType": "max",
+            "constraints": constraints, "variables": variables, "ints": {f"x{i}": 1 for i in range(n_ints)}}
+
+
 # ---- the reference's stress families (solver.stress.test.ts:41-215 solves them at 10..50 variables) ----------
 # Same shapes and distributions as problem-generator.ts's families, drawn from numpy's stream; every model is a
 # plain jsLPSolver JSON dict, so every implementation that is compared (and an outside solver) sees the same instance.

@@ -369,7 +369,7 @@ class RefModel:
         opt: dict[int, np.ndarray] = {}
         col_of: dict[int, int] = {}
         for v, var in enumerate(self.variables):
-            cost = coeff * var.cost
+            cost = coeff * float(var.cost)   # a double product, as in JS: -1 * 0 is -0
             if var.priority == 0:
                 M[0, v + 1] = cost
             else:
@@ -387,8 +387,8 @@ class RefModel:
                 M[r, 0] = c.rhs
             else:
                 for t in c.terms:
-                    M[r, col_of[t.variable.index]] = -t.coefficient
-                M[r, 0] = -c.rhs
+                    M[r, col_of[t.variable.index]] = -float(t.coefficient)
+                M[r, 0] = -float(c.rhs)
             r += 1
         prios = sorted(opt.keys())
         rc = np.stack([opt[p] for p in prios]) if prios else np.zeros((0, W))

@@ -18,11 +18,13 @@ ENGINES = {"two_kernel": 1, "fused": 2, "resident": 4, "fused_generic_tail": (2,
 
 
 def same_bits(a, b):
+    """Bit for bit: -0.0 differs from +0.0 (JS sees the sign through 1 / x and Math.min), any NaN equals any NaN (JS
+    cannot observe a NaN's payload)."""
     a = np.ascontiguousarray(a, dtype=np.float64)
     b = np.ascontiguousarray(b, dtype=np.float64)
     if a.shape != b.shape:
         return False
-    return bool(np.all((a == b) | (np.isnan(a) & np.isnan(b))))
+    return bool(np.all((a.view(np.uint64) == b.view(np.uint64)) | (np.isnan(a) & np.isnan(b))))
 
 
 def oracle_lp(it, precision=1e-8, check_cycles=True, log=1 << 16):
@@ -86,6 +88,17 @@ def assert_lp_parity(g, o, what=""):
         assert same_bits(st.evaluation, os_.evaluation), what
     if g.nOpt:
         assert same_bits(g.optional_reduced_costs(), o.optional()), what
+
+
+def assert_node_log_parity(gt, ot, what=""):
+    """Branch-and-cut node logs of the device tableau gt and the oracle tableau ot: same nodes in the same order, same
+    integer fields, and the bits of the relaxed evaluation and (for a feasible node) the evaluation."""
+    onl, gnl = ot.node_log(), gt.node_log()
+    assert gnl.shape == onl.shape, (what, gnl.shape, onl.shape)
+    for i in range(len(onl)):
+        a, b = gnl[i], onl[i]
+        ok = all(a[k] == b[k] for k in (0, 1, 2, 4, 5, 7)) and same_bits(a[6], b[6]) and (not b[2] or same_bits(a[3], b[3]))
+        assert ok, f"{what} node {i}: gpu={a.tolist()} oracle={b.tolist()}"
 
 
 # ------------------------------------------------------------------ golden fixtures end to end
@@ -274,9 +287,43 @@ BNB_MODES = {"hbm_seq": (2, 1), "auto_seq": (0, 1), "auto_spec8": (0, 8), "auto_
              "auto_spec8_logcap3": (0, 8, None, None, {14: 3})}
 
 
+def _generated_mips():
+    """Branch-and-cut inputs built by problems.half_tie_mip_model, in the shape of a fixture: the LP relaxation keeps
+    most basic integer variables at exactly k + 1/2, so the position tie-break picks the branching variable at nearly
+    every node.  80 integer rows (the root and its nodes fit the shared-memory node kernel, integer rows in three
+    warps) and 300 (past one 256-thread pass of the MIP scan; the HBM path and node slots).  max_nodes caps the loop."""
+    from jslpsolver_b200 import problems
+    return [{"file": f"half_tie_{n}", "model": problems.half_tie_mip_model(n, seed=n), "max_nodes": cap, "k2": n == 80}
+            for n, cap in ((80, 120), (300, 40))]
+
+
+GENERATED_MIPS = _generated_mips()
+MIP_FIXTURES = [f for f in BUNDLE["fixtures"] if (f["model"].get("ints") or f["model"].get("binaries"))]
+GENERATED_MODES = ("hbm_seq", "auto_spec8", "hbm_spec4", "hbm_slots3_steps5", "auto_spec8_logcap3")
+
+
+def solve_capped(s, jm, max_nodes=0):
+    """s.Solve(jm, full=True) with the branch-and-cut loop stopped after max_nodes nodes (0 = no cap)."""
+    inst = s._instance(jm, None)
+    inst.max_nodes = max_nodes
+    return s._finish(inst, inst.solve(), True)
+
+
+def assert_backend(gt, fx, mode):
+    """A generated MIP reached the back end its mode names: the shared-memory node kernel (automatic engine, nodes
+    that fit), node slots (speculated rounds of nodes that do not, or engine 2), or neither (one node at a time)."""
+    b = gt.lastBnbStatus
+    print(f"{fx['file']} {mode}: nodes {b.iterations} node kernel {b.node_kernel_ms:.3f} ms slot pivots {b.slot_pivots}")
+    if mode == "hbm_seq":
+        assert b.node_kernel_ms == 0 and b.slot_pivots == 0, (mode, b.node_kernel_ms, b.slot_pivots)
+    elif mode.startswith("auto") and fx["k2"]:
+        assert b.node_kernel_ms > 0, (mode, b.node_kernel_ms)
+    else:
+        assert b.node_kernel_ms == 0 and b.slot_pivots > 0, (mode, b.node_kernel_ms, b.slot_pivots)
+
+
 @pytest.mark.parametrize("mode", list(BNB_MODES))
-@pytest.mark.parametrize("fx", [f for f in BUNDLE["fixtures"] if (f["model"].get("ints") or f["model"].get("binaries"))],
-                         ids=lambda f: f["file"])
+@pytest.mark.parametrize("fx", MIP_FIXTURES + GENERATED_MIPS, ids=lambda f: f["file"])
 def test_mip_fixture_node_sequence(fx, mode):
     """Same pop order, same per-node outcomes, same final tableau as the reference's loop --
     whatever the speculation width or evaluation back-end."""
@@ -286,8 +333,11 @@ def test_mip_fixture_node_sequence(fx, mode):
         pytest.skip("large MIP: covered by two modes")
     if fx["file"] == "Vendor Selection.json" and mode != "auto_spec32":
         pytest.skip("long MIP: covered by one mode")
+    if "k2" in fx and mode not in GENERATED_MODES:
+        pytest.skip("generated MIP: covered by one mode per back end")
     jm = strip_timeouts(fx["model"])
-    osol = ref_model.solve_full(jm, fast_cycles=True, node_log=1 << 20)
+    max_nodes = fx.get("max_nodes", 0)
+    osol = ref_model.solve_full(jm, fast_cycles=True, node_log=1 << 20, max_nodes=max_nodes)
     if osol.tableau is None:
         pytest.skip("decided by presolve")
     s = J.Solver()
@@ -296,15 +346,11 @@ def test_mip_fixture_node_sequence(fx, mode):
         s.node_slots, s.slot_steps = BNB_MODES[mode][2:4]
     if len(BNB_MODES[mode]) > 4:
         s.options = dict(BNB_MODES[mode][4])
-    gsol = s.Solve(jm, full=True)
+    gsol = solve_capped(s, jm, max_nodes)
     gt = gsol._tableau
-    onl, gnl = osol.tableau.node_log(), gt.node_log()
-    assert gnl.shape == onl.shape, (gnl.shape, onl.shape)
-    for i in range(len(onl)):
-        a, b = gnl[i], onl[i]
-        ok = a[0] == b[0] and a[1] == b[1] and a[2] == b[2] and a[4] == b[4] and a[5] == b[5] and a[7] == b[7]
-        ok = ok and same_bits(a[6], b[6]) and (not b[2] or same_bits(a[3], b[3]))
-        assert ok, f"node {i}: gpu={a.tolist()} oracle={b.tolist()}"
+    assert_node_log_parity(gt, osol.tableau, fx["file"])
+    if "k2" in fx:
+        assert_backend(gt, fx, mode)
     st = osol.state
     assert gt.branchAndCutIterations == st.bncIterations
     assert (gt.feasible, gt.bounded) == (bool(st.feasible), bool(st.bounded))
@@ -396,27 +442,25 @@ def test_mir_primitives_match_oracle():
     assert g.height == o.state().height and same_bits(g.matrix2d(), o.matrix())
 
 
-@pytest.mark.parametrize("fx", [f for f in BUNDLE["fixtures"] if (f["model"].get("ints") or f["model"].get("binaries"))],
-                         ids=lambda f: f["file"])
+@pytest.mark.parametrize("fx", MIP_FIXTURES + GENERATED_MIPS, ids=lambda f: f["file"])
 def test_mip_fixture_with_mir_cuts_matches_oracle(fx):
     """options.useMIRCuts: same node sequence, same final tableau as the oracle's restatement of the MIR loop."""
     import jslpsolver_b200 as J
     from oracle import ref_model
     jm = strip_timeouts(fx["model"])
     jm["options"] = dict(jm.get("options") or {}, useMIRCuts=True)
-    osol = ref_model.solve_full(jm, fast_cycles=True, node_log=1 << 20)
+    max_nodes = fx.get("max_nodes", 0)
+    osol = ref_model.solve_full(jm, fast_cycles=True, node_log=1 << 20, max_nodes=max_nodes)
     if osol.tableau is None:
         pytest.skip("decided by presolve")
     s = J.Solver()
     s.max_spec_batch = 8
-    gsol = s.Solve(jm, full=True)
+    gsol = solve_capped(s, jm, max_nodes)
     gt = gsol._tableau
-    onl, gnl = osol.tableau.node_log(), gt.node_log()
-    assert gnl.shape == onl.shape, (gnl.shape, onl.shape)
-    for i in range(len(onl)):
-        a, b = gnl[i], onl[i]
-        ok = all(a[k] == b[k] for k in (0, 1, 2, 4, 5, 7)) and same_bits(a[6], b[6]) and (not b[2] or same_bits(a[3], b[3]))
-        assert ok, f"node {i}: gpu={a.tolist()} oracle={b.tolist()}"
+    assert_node_log_parity(gt, osol.tableau, fx["file"])
+    if "k2" in fx:   # the MIR loop runs on the single-tableau path: neither the node kernel nor node slots
+        b = gt.lastBnbStatus
+        assert b.node_kernel_ms == 0 and b.slot_pivots == 0, (b.node_kernel_ms, b.slot_pivots)
     assert gt.branchAndCutIterations == osol.state.bncIterations
     assert same_bits(gt.matrix2d(), osol.tableau.matrix())
     assert np.array_equal(gt.varIndexByRow, osol.tableau.maps()[0])
@@ -569,8 +613,7 @@ ENHANCED = [{"nodeSelection": "hybrid"}, {"nodeSelection": "depth-first", "branc
 
 
 @pytest.mark.parametrize("opts", ENHANCED, ids=lambda o: "-".join(str(v) for v in o.values()))
-@pytest.mark.parametrize("fx", [f for f in BUNDLE["fixtures"] if (f["model"].get("ints") or f["model"].get("binaries"))],
-                         ids=lambda f: f["file"])
+@pytest.mark.parametrize("fx", MIP_FIXTURES + GENERATED_MIPS, ids=lambda f: f["file"])
 def test_enhanced_service_matches_oracle(fx, opts):
     """options.nodeSelection / options.branching select the enhanced service (main.ts:62-83): same node sequence (stack /
     heap order, pseudocost-driven branching variables), same final tableau as the oracle's restatement."""
@@ -578,20 +621,18 @@ def test_enhanced_service_matches_oracle(fx, opts):
     from oracle import ref_model
     if fx["file"] in ("Vendor Selection.json", "Monster_II.json") and "branching" in opts and opts.get("nodeSelection") != "depth-first":
         pytest.skip("long MIP: covered by two combinations")
+    if "k2" in fx and opts != ENHANCED[0]:
+        pytest.skip("generated MIP: covered by the hybrid / pseudocost service")
     jm = strip_timeouts(fx["model"])
     jm["options"] = dict(jm.get("options") or {}, **opts)
-    osol = ref_model.solve_full(jm, fast_cycles=True, node_log=1 << 20)
+    max_nodes = fx.get("max_nodes", 0)
+    osol = ref_model.solve_full(jm, fast_cycles=True, node_log=1 << 20, max_nodes=max_nodes)
     if osol.tableau is None:
         pytest.skip("decided by presolve")
     s = J.Solver()
-    gsol = s.Solve(jm, full=True)
+    gsol = solve_capped(s, jm, max_nodes)
     gt = gsol._tableau
-    onl, gnl = osol.tableau.node_log(), gt.node_log()
-    assert gnl.shape == onl.shape, (gnl.shape, onl.shape)
-    for i in range(len(onl)):
-        a, b = gnl[i], onl[i]
-        ok = all(a[k] == b[k] for k in (0, 1, 2, 4, 5, 7)) and same_bits(a[6], b[6]) and (not b[2] or same_bits(a[3], b[3]))
-        assert ok, f"node {i}: gpu={a.tolist()} oracle={b.tolist()}"
+    assert_node_log_parity(gt, osol.tableau, fx["file"])
     assert gt.branchAndCutIterations == osol.state.bncIterations
     assert same_bits(gt.matrix2d(), osol.tableau.matrix())
     assert s._simplified(gsol) == ref_model.simplify(osol)

@@ -119,25 +119,29 @@ def mixed_arrays(n_rows, n_vars, seed, n_lower=4, profitable=None):
     return A, b, c, lower
 
 
-def tie_arrays(n_rows, n_vars, seed, G, nt, profitable=None):
+def tie_arrays(n_rows, n_vars, seed, G, nt, profitable=None, row_offsets=None, col_offsets=None):
     """mixed_arrays with exact ties where the device merges partial results.  Rows: lanes 2..9 of row CTA 1 are copied
     to the same lanes of three other row CTAs (equal ratio-test quotients merged across CTAs; after a pivot on one copy
     the others are degenerate in several CTAs).  Columns: the most profitable column is copied 50 columns on (the next
     partial-pricing batch) and 8 x threads columns on (another register slot of the selector).  Row CTA b of G owns
-    tableau rows from b * (H // G) + min(b, H % G)."""
+    tableau rows from b * (H // G) + min(b, H % G).  row_offsets / col_offsets replace those placements for a kernel
+    that splits the tableau differently: tableau rows 2..9 are copied that many rows on, the column that many columns
+    on."""
     A, b, c, lower = mixed_arrays(n_rows, n_vars, seed, n_lower=2, profitable=profitable)
     H = n_rows + 1
     base, rem = divmod(H, G)
     r0 = lambda k: k * base + min(k, rem)
     lanes = range(2, min(10, base))
-    for k in sorted({3 % G, G // 2, G - 1} - {1}):
-        for lane in lanes:
-            src, dst = r0(1) + lane - 1, r0(k) + lane - 1   # tableau row t is array row t - 1
-            if 0 <= dst < n_rows and dst != src:
-                A[dst], b[dst], lower[dst] = A[src], b[src], lower[src]
+    if row_offsets is None:
+        pairs = [(r0(1) + lane - 1, r0(k) + lane - 1) for k in sorted({3 % G, G // 2, G - 1} - {1}) for lane in lanes]
+    else:
+        pairs = [(t - 1, t - 1 + off) for off in row_offsets for t in range(2, 10)]
+    for src, dst in pairs:   # tableau row t is array row t - 1
+        if 0 <= dst < n_rows and dst != src:
+            A[dst], b[dst], lower[dst] = A[src], b[src], lower[src]
     j0 = 1
     c[j0] = c.max() + 1.0
-    for off in (50, 8 * nt):
+    for off in (50, 8 * nt) if col_offsets is None else col_offsets:
         if j0 + off < n_vars:
             A[:, j0 + off], c[j0 + off] = A[:, j0], c[j0]
     return A, b, c, lower

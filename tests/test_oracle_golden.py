@@ -394,3 +394,15 @@ def test_oracle_verdicts_equal_an_independent_solver_on_mixed_models():
             assert not (res["feasible"] and res["bounded"]), (k, res)
         seen[status] = seen.get(status, 0) + 1
     assert seen[0] >= 40 and seen[2] >= 40 and seen[3] >= 15, seen
+
+
+def test_oracle_root_tableau_is_the_front_ends_bit_for_bit():
+    """Tableau.setModel (tableau.ts:332-378) in the oracle and in the front end: every fixture's root tableau has the
+    same bits, signed zeros included (JS stores -1 * 0 and -(0) as -0 in the cost row and in `min` rows)."""
+    from jslpsolver_b200.model import Model
+    from oracle.ref_model import RefModel
+    for fx in load_bundle()["fixtures"]:
+        jm = strip_timeouts(fx["model"])
+        a = Model().loadJson(jm).initial_tableau().matrix
+        b = RefModel(None).loadJson(jm).build_tableau()[0]
+        assert a.shape == b.shape and np.array_equal(a.view(np.uint64), b.view(np.uint64)), fx["file"]

@@ -63,17 +63,13 @@ def test_oracle_agrees_with_an_independent_solver(label, model):
         assert status in (3, 4) and not (res["feasible"] and res["bounded"]), (label, status, res)
 
 
-def same_bits(a, b):
-    a, b = np.ascontiguousarray(a, dtype=np.float64), np.ascontiguousarray(b, dtype=np.float64)
-    return a.shape == b.shape and np.array_equal(a.view(np.uint64), b.view(np.uint64))
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("spec", [1, 8, 32, "hbm_slots"])
 @pytest.mark.parametrize("label,model", SUITE, ids=[s[0] for s in SUITE])
 def test_gpu_matches_oracle_bit_for_bit(label, model, spec):
     import jslpsolver_b200 as J
     from oracle import ref_model
+    from test_gpu_lp_parity import same_bits
     is_mip = bool(model.get("ints") or model.get("binaries"))
     if not is_mip and spec != 1:
         pytest.skip("speculation width only matters with integer variables")
