@@ -246,6 +246,14 @@ int jslp_scenario_batch(jslp_tab *tab, const jslp_scenario_edit *edits, const in
                         int check_cycles, int32_t *status, double *eval_raw, int32_t *p1, int32_t *p2, double *rhs,
                         int32_t *vrow);
 
+/* Warm-start crash, DESIGN.md section 2f: for each label enter[k] in order, pivot it into the basis on the row with the
+ * largest |M[r,c]| among the rows r >= 1 whose basic label l has leave[l] != 0 and M[r,c] < -P || P < M[r,c] (lowest
+ * row on ties); leave has one byte per label (n_index, see jslp_tab_info).  out[4k .. 4k+3] = (label, row, column,
+ * leaving label) of a pivot, (label, row, -1, -2) when the label is already basic, (label, -1, column, -1) when no row
+ * is eligible.  n_pivots = pivots done.  The tableau, labels and pivot record are left as the same jslp_pivot calls
+ * would leave them; the crash pivots are not added to the pivot log.  No optional objectives. */
+int jslp_crash(jslp_tab *tab, const int32_t *enter, int n_enter, const uint8_t *leave, int32_t *out, int *n_pivots);
+
 /* Multi-GPU communicator of the branch-and-cut frontier (one process per GPU).  NCCL is loaded at run time;
  * without libnccl these calls fail with JSLP_E_UNSUPPORTED and single-GPU use is unaffected.  Rank 0 obtains a
  * 128-byte unique id and hands it to the other ranks through whatever bootstrap the host has (the N-API host:

@@ -175,6 +175,10 @@ struct jslp_tab {
     int param_cap = 0;
     cudaGraphExec_t param_graph = nullptr;
     int param_key[3] = {0, 0, 0};  // step grid, shared memory and variant the graph was captured for
+    void *d_crash = nullptr, *d_crash_buf = nullptr;  // jslp_crash: list state; records, labels and leave mask
+    size_t crash_bytes = 0;
+    cudaGraphExec_t crash_graph = nullptr;
+    int crash_key[3] = {0, 0, 0};
 };
 
 extern "C" const char *jslp_last_error(void) { return g_err.c_str(); }
@@ -342,6 +346,8 @@ extern "C" void jslp_tab_destroy(jslp_tab *t) {
     cudaFree(t->d_sens); cudaFree(t->d_iis); cudaFree(t->d_scen);
     cudaFree(t->d_param); cudaFree(t->d_plog);
     if (t->param_graph) cudaGraphExecDestroy(t->param_graph);
+    cudaFree(t->d_crash); cudaFree(t->d_crash_buf);
+    if (t->crash_graph) cudaGraphExecDestroy(t->crash_graph);
     free_saved(t->saved);
     free_snap(t->snaps[0]);
     free_snap(t->snaps[1]);
@@ -1363,3 +1369,4 @@ extern "C" int jslp_pivot_log(jslp_tab *t, int32_t *entries, int cap, int *n) {
 #include "jslp_iis.cuh"
 #include "jslp_parametric.cuh"
 #include "jslp_scenario.cuh"
+#include "jslp_crash.cuh"

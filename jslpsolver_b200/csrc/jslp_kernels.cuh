@@ -223,6 +223,16 @@ __device__ __forceinline__ void param_ratio(int i, double num, double den, bool 
     if (q < best.v) { best.v = q; best.i = i; }
 }
 
+// One row of the warm-start crash (DESIGN.md section 2f): a row whose basic label the saved basis gives up (`leave`)
+// takes part when its entry v in the entering column passes putInBase's test v < -prec || prec < v (a NaN never does),
+// and the largest |v| wins (lowest row on ties when rows come in increasing order).  |v| of a candidate is positive and
+// finite or +inf, so the double itself is an order-preserving key for block_reduce_vi.
+__device__ __forceinline__ void crash_step(int r, double v, bool leave, double prec, VI &best) {
+    if (!leave || !(v < -prec || prec < v)) return;
+    const double key = fabs(v);
+    if (key > best.v) { best.v = key; best.i = r; }
+}
+
 // The dynamic-modification edits (dynamic-modification.ts:78-160), each one entry: x - d * y and x + d * y (difference
 // times entry, then subtract / add: two roundings), and x - d.  updateRightHandSide and updateCost are built from these
 // three, on the HBM tableau (jslp_dynamic.cuh) and in the scenario prologue of k_node_batch alike.

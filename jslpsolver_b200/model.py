@@ -428,7 +428,10 @@ class Model:
         return InitialTableau(M, vrow, vcol, unres, ints, prios, costs)
 
     # ------------------------------------------------------------------ solve (model.ts:427-467)
-    def solve(self):
+    def solve(self, *, basis=None):
+        if basis is not None:  # warm start from a saved basis (DESIGN.md section 2f)
+            from .warmstart import solve
+            return solve(self, basis)
         if self.usePresolve and self.presolveResult is None:
             self.presolveResult = presolve(self)
             if self.presolveResult.isInfeasible:

@@ -20,7 +20,10 @@ class Solver:
         self.slot_steps = None
         self.options: dict = {}    # JSLP_OPT_* -> value for every tableau this solver creates (tuning / test aids)
 
-    def Solve(self, model: Any, precision: Optional[float] = None, full: bool = False, validate: bool = False):
+    def Solve(self, model: Any, precision: Optional[float] = None, full: bool = False, validate: bool = False, *,
+              basis: Optional[dict] = None):
+        if basis is not None:  # warm start from a saved basis (DESIGN.md section 2f)
+            return self._solve_warm(model, precision, full, validate, basis)
         if validate:
             model = validation.validate(model)  # main.ts:101-108
         if not model:
@@ -33,6 +36,22 @@ class Solver:
                 raise NotImplementedError("external solvers (src/external) are out of scope")
         instance = self._instance(model, precision)
         solution = instance.solve()
+        return self._finish(instance, solution, full)
+
+    def _solve_warm(self, model: Any, precision: Optional[float], full: bool, validate: bool, basis: dict):
+        from .warmstart import WHAT
+        if validate:
+            model = validation.validate(model)
+        if not model:
+            raise ValueError("Solver requires a model to operate on")
+        if isinstance(model, dict):
+            opt = model.get("optimize")
+            if isinstance(opt, dict) and len(opt) > 1:
+                raise ValueError(f"{WHAT} does not support multi-objective models (optimize with several objectives)")
+            if model.get("external"):
+                raise NotImplementedError("external solvers (src/external) are out of scope")
+        instance = self._instance(model, precision)
+        solution = instance.solve(basis=basis)
         return self._finish(instance, solution, full)
 
     def MultiObjective(self, model: dict):  # main.ts:209-211
@@ -83,5 +102,6 @@ class Solver:
 solver = Solver()
 
 
-def Solve(model: Any, precision: Optional[float] = None, full: bool = False, validate: bool = False):
-    return solver.Solve(model, precision, full, validate)
+def Solve(model: Any, precision: Optional[float] = None, full: bool = False, validate: bool = False, *,
+          basis: Optional[dict] = None):
+    return solver.Solve(model, precision, full, validate, basis=basis)

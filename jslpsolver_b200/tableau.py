@@ -86,6 +86,15 @@ class Solution:  # solution.ts:16-61
         self._version = getattr(tableau, "_version", None)  # the tableau state this solution describes
         self.solutionSet: dict = {}
 
+    warmStart = None  # Solve(model, full=True, basis=...): what the crash did (DESIGN.md section 2f)
+
+    def basis(self) -> dict:
+        """The basis of this continuous LP optimum as JSON-serialisable names, {"variables": [basic variable ids],
+        "constraints": [{"name", "type"} of the binding rows]}, for Solve(model, basis=...) (DESIGN.md section 2f);
+        raises ValueError where sensitivity() does."""
+        from .warmstart import basis
+        return basis(self)
+
     def sensitivity(self) -> dict:
         """Shadow prices, reduced costs and right-hand-side / cost ranges of this continuous LP optimum
         (DESIGN.md section 2b); raises ValueError where they are not defined."""
@@ -659,6 +668,21 @@ class GpuTableau:
             self._h(), arr, off.ctypes.data, n, cc, status.ctypes.data, eval_raw.ctypes.data, p1.ctypes.data,
             p2.ctypes.data, rhs.ctypes.data, vrow.ctypes.data))
         return {"status": status, "eval_raw": eval_raw, "p1": p1, "p2": p2, "rhs": rhs, "vrow": vrow}
+
+    def crash(self, enter, leave):
+        """jslp_crash: pivot the labels `enter` into the basis in order, each on the row with the largest |entry| among
+        the rows whose basic label has leave[label] != 0 (DESIGN.md section 2f).  Returns the records (n x 4: label,
+        row, column, leaving label or -1 rejected / -2 already basic) and the number of pivots done."""
+        ent = np.ascontiguousarray(enter, dtype=np.int32)
+        lv = np.ascontiguousarray(leave, dtype=np.uint8)
+        if len(lv) != self.nVars:
+            raise ValueError(f"crash: the leave mask has {len(lv)} entries, the tableau {self.nVars} labels")
+        out = np.empty((max(1, len(ent)), 4), dtype=np.int32)
+        n = C.c_int()
+        _lib.check(self.context.lib.jslp_crash(self._h(), ent.ctypes.data if len(ent) else None, len(ent),
+                                               lv.ctypes.data if len(lv) else None, out.ctypes.data, C.byref(n)))
+        self._edited()
+        return out[:len(ent)], n.value
 
     def optional_reduced_costs(self) -> np.ndarray:
         return self._download("opt")
