@@ -254,6 +254,25 @@ int jslp_scenario_batch(jslp_tab *tab, const jslp_scenario_edit *edits, const in
  * would leave them; the crash pivots are not added to the pivot log.  No optional objectives. */
 int jslp_crash(jslp_tab *tab, const int32_t *enter, int n_enter, const uint8_t *leave, int32_t *out, int *n_pivots);
 
+/* Pareto frontier of two objectives from the current (optimal) tableau of the first, DESIGN.md section 2g: the second
+ * objective's row is priced against the basis, then the weight theta of (1 - theta) * first + theta * second moves from
+ * 0 to 1 with one pivot per basis change (the cost path of section 2d along the carried direction E = R2 - row 0).
+ *   cost2_by_label  n_index entries (see jslp_tab_info): sigma2 * c2_j at each structural label, 0 elsewhere
+ *   r2 / dir        width entries: the priced second objective R2 and the direction E at theta = 0
+ *   theta .. rc_lbl, n_breaks, stop   the breakpoint records and the stop code as jslp_parametric writes them
+ *                   (max_breaks entries; stop 1 reached theta = 1, 3 unbounded beyond theta, 4 max_breaks pieces)
+ *   pt_rhs / pt_vrow / pt_break   per point k < min(n_points, max_points): column 0 and the row labels (height
+ *                   entries each at k * height) and the number of records before it (0 = the start); a point is
+ *                   appended after every pivot that changes column 0 (M[r*,0] != 0), and the last one is the end
+ *   n_points        points on the whole path (may exceed max_points: call again with more room)
+ *   end_rhs / end_vrow  height entries: column 0 and the row labels at the end of the path
+ * The tableau, its labels, the staged pivot, the pivot record and the descriptor (no optional objectives) are restored
+ * before the call returns.  No optional objectives. */
+int jslp_frontier(jslp_tab *tab, const double *cost2_by_label, int max_breaks, int max_points, double *r2, double *dir,
+                  double *theta, double *obj_raw, double *dobj, int32_t *rc_lbl, int *n_breaks, int *stop,
+                  double *pt_rhs, int32_t *pt_vrow, int32_t *pt_break, int *n_points, double *end_rhs,
+                  int32_t *end_vrow);
+
 /* Multi-GPU communicator of the branch-and-cut frontier (one process per GPU).  NCCL is loaded at run time;
  * without libnccl these calls fail with JSLP_E_UNSUPPORTED and single-GPU use is unaffected.  Rank 0 obtains a
  * 128-byte unique id and hands it to the other ranks through whatever bootstrap the host has (the N-API host:

@@ -175,6 +175,8 @@ struct jslp_tab {
     int param_cap = 0;
     cudaGraphExec_t param_graph = nullptr;
     int param_key[3] = {0, 0, 0};  // step grid, shared memory and variant the graph was captured for
+    void *d_front = nullptr;  // jslp_frontier: second objective, priced row, carried direction and point slots
+    size_t front_bytes = 0;
     void *d_crash = nullptr, *d_crash_buf = nullptr;  // jslp_crash: list state; records, labels and leave mask
     size_t crash_bytes = 0;
     cudaGraphExec_t crash_graph = nullptr;
@@ -344,7 +346,7 @@ extern "C" void jslp_tab_destroy(jslp_tab *t) {
     cudaFreeHost(t->h_rec); cudaFreeHost(t->h_log); cudaFreeHost(t->h_mip); cudaFreeHost(t->h_cuts);
     cudaFree(t->d_count); cudaFreeHost(t->h_count);
     cudaFree(t->d_sens); cudaFree(t->d_iis); cudaFree(t->d_scen);
-    cudaFree(t->d_param); cudaFree(t->d_plog);
+    cudaFree(t->d_param); cudaFree(t->d_plog); cudaFree(t->d_front);
     if (t->param_graph) cudaGraphExecDestroy(t->param_graph);
     cudaFree(t->d_crash); cudaFree(t->d_crash_buf);
     if (t->crash_graph) cudaGraphExecDestroy(t->crash_graph);
@@ -1370,3 +1372,4 @@ extern "C" int jslp_pivot_log(jslp_tab *t, int32_t *entries, int cap, int *n) {
 #include "jslp_parametric.cuh"
 #include "jslp_scenario.cuh"
 #include "jslp_crash.cuh"
+#include "jslp_frontier.cuh"

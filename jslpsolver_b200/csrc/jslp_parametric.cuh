@@ -10,6 +10,9 @@
 //                  is non-basic.  Step bound t* = min of -M[0,c] / E[c] over restricted columns with E[c] > P;
 //                  shift M[0,c] += t * E[c]; the entering column c* gets M[0,c*] = +0; leaving row = the reference's
 //                  phase-2 ratio test on c* (ratio_step).
+//   frontier (kind 2)  as kind 1 with E read from the descriptor's one optional-objective row, which the step carries
+//                  through every pivot (jslp_frontier.cuh, section 2g); each call first appends the current point
+//                  (column 0 and the row labels) to a per-poll slot when the previous pivot changed it.
 //
 // sign_i = g * s_i (rhs) or g * sigma (cost), g = +1 when the target lies above the start.  The pivot itself is the
 // two-kernel engine's: k_param_select stages it exactly as k_select stages Tableau.pivot(), and the in-place step
@@ -36,6 +39,11 @@ struct ParamDev {
     double sign[2];
     double g, target, theta;
     int status, n, max_breaks, pad;
+    // kind 2: PARAM_STEPS point slots of rowcap entries each, the record count at which each point was appended, the
+    // points appended so far and whether the last staged pivot leaves a non-zero M[r*,0] (it changes the point)
+    double *pt_rhs;
+    int *pt_vrow, *pt_at;
+    int npts, moved;
 };
 
 struct ParamSmem {
@@ -68,6 +76,16 @@ __global__ void __launch_bounds__(512) k_param_select(const TabDev *Tp, Rec *rec
     if (tid < 2) { s.row[tid] = -1; s.col[tid] = -1; }
     __syncthreads();
     if (P.status != PAR_RUNNING) return;
+    if (P.kind == 2 && P.moved) {  // the point the previous pivot moved to (or the start), before anything shifts
+        const int slot = P.npts % PARAM_STEPS;
+        const size_t off = (size_t)slot * T.rowcap;
+        for (int r = tid; r < T.H; r += NT) {
+            P.pt_rhs[off + r] = ldg_cg(T.M + (size_t)r * T.stride);
+            P.pt_vrow[off + r] = T.vrow[r];
+        }
+        if (tid == 0) { P.pt_at[slot] = P.n; Pp->npts = P.npts + 1; Pp->moved = 0; }
+        __syncthreads();
+    }
     if (P.n >= P.max_breaks) {
         if (tid == 0) Pp->status = PAR_LIMIT;
         return;
@@ -190,10 +208,11 @@ __global__ void __launch_bounds__(512) k_param_select(const TabDev *Tp, Rec *rec
         return;
     }
 
-    // ---- cost: step bound over the columns, E kept in prow
+    // ---- cost: step bound over the columns, E kept in prow (kind 2: E is the carried row T.opt)
     const int rv_ = s.row[0], cv_ = s.col[0];
     const double sg = P.sign[0];
-    const double *vr = rv_ >= 0 ? M + rv_ * stride : nullptr;
+    const bool carried = P.kind == 2;
+    const double *vr = carried ? T.opt : (rv_ >= 0 ? M + rv_ * stride : nullptr);
     VI best = init;
     for (int c0 = 0; c0 < W; c0 += 8 * NT) {
         double m0[8], er[8];
@@ -209,7 +228,7 @@ __global__ void __launch_bounds__(512) k_param_select(const TabDev *Tp, Rec *rec
         for (int k = 0; k < 8; k++) {
             const int c = c0 + tid + k * NT;
             if (c >= W) continue;
-            const double e = vr != nullptr ? __dmul_rn(-sg, er[k]) : (c == cv_ ? sg : 0.0);
+            const double e = carried ? er[k] : (vr != nullptr ? __dmul_rn(-sg, er[k]) : (c == cv_ ? sg : 0.0));
             T.prow[c] = e;
             if (c == 0) s.d0 = e;
             else param_ratio(c, m0[k], -e, is_unres(T, lab[k]), prec, best);
@@ -272,7 +291,10 @@ __global__ void __launch_bounds__(512) k_param_select(const TabDev *Tp, Rec *rec
         return;
     }
     __syncthreads();  // every read of the direction in prow is done before the pivot row replaces it
-    if (tid == 0) param_record(Pp, P, theta, s.obj, s.d0, rstar, cstar, T.vrow[rstar], T.vcol[cstar], PAR_RUNNING);
+    if (tid == 0) {
+        param_record(Pp, P, theta, s.obj, s.d0, rstar, cstar, T.vrow[rstar], T.vcol[cstar], PAR_RUNNING);
+        if (carried) Pp->moved = ldg_cg(M + rstar * stride) != 0.0;
+    }
     cta_stage_pivot(T, rec, 2, rstar, cstar, isneg ? 1 : 0, cnt);
 }
 
@@ -312,8 +334,11 @@ static int param_graph(jslp_tab *t, cudaGraphExec_t *out) {
     return JSLP_OK;
 }
 
-// The path on the live tableau; the caller snapshots it before and restores it after.
-static int parametric_run(jslp_tab *t, const ParamDev &p, int *n_out, int *status_out, double *end_rhs, int32_t *end_vrow) {
+// The path on the live tableau; the caller snapshots it before and restores it after.  `drain`, when given, runs after
+// every poll with the path state as the poll read it (jslp_frontier collects its point slots there).
+typedef int (*param_drain_fn)(jslp_tab *t, const ParamDev &cur, void *arg);
+static int parametric_run(jslp_tab *t, const ParamDev &p, int *n_out, int *status_out, double *end_rhs, int32_t *end_vrow,
+                          param_drain_fn drain = nullptr, void *drain_arg = nullptr) {
     jslp_ctx *ctx = t->ctx;
     cudaStream_t s = ctx->stream;
     Rec init;
@@ -332,6 +357,10 @@ static int parametric_run(jslp_tab *t, const ParamDev &p, int *n_out, int *statu
         ctx->launches += 1 + 2 * PARAM_STEPS;
         CK(cudaMemcpyAsync(&cur, t->d_param, sizeof(ParamDev), cudaMemcpyDeviceToHost, s));
         CK(cudaStreamSynchronize(s));
+        if (drain) {
+            const int rc = drain(t, cur, drain_arg);
+            if (rc) return rc;
+        }
     }
     // the end state, before the caller restores the tableau
     CK(cudaMemcpy2DAsync(end_rhs, sizeof(double), t->hd.M, sizeof(double) * t->stride, sizeof(double), t->H,

@@ -5,6 +5,7 @@ from __future__ import annotations
 from typing import Any, Optional
 
 from . import validation
+from .frontier import Frontier as _frontier
 from .model import Model, object_keys
 from .polyopt import Polyopt
 
@@ -57,6 +58,11 @@ class Solver:
     def MultiObjective(self, model: dict):  # main.ts:209-211
         return Polyopt(self, model)
 
+    def Frontier(self, model: dict, precision: Optional[float] = None, validate: bool = False) -> dict:
+        """The Pareto frontier of a continuous LP with exactly two objectives: every efficient vertex from the first
+        objective's optimum to the second's, with the weights that select it (frontier.py, DESIGN.md section 2g)."""
+        return _frontier(self, model, precision, validate)
+
     def _instance(self, model: Any, precision: Optional[float]) -> Model:
         if isinstance(model, dict):
             options = model.get("options") or {}
@@ -105,3 +111,7 @@ solver = Solver()
 def Solve(model: Any, precision: Optional[float] = None, full: bool = False, validate: bool = False, *,
           basis: Optional[dict] = None):
     return solver.Solve(model, precision, full, validate, basis=basis)
+
+
+def Frontier(model: dict, precision: Optional[float] = None, validate: bool = False) -> dict:
+    return solver.Frontier(model, precision, validate)

@@ -649,6 +649,39 @@ class GpuTableau:
         return {"theta": theta[:k], "obj_raw": obj[:k], "dobj": dobj[:k], "rc_lbl": rc[:k], "stop": stop.value,
                 "end_rhs": end_rhs, "end_vrow": end_vrow}
 
+    def frontier_path(self, cost2_by_label, max_breaks: int, max_points: Optional[int] = None) -> dict:
+        """jslp_frontier: the second objective priced against the current optimal tableau (R2 and the direction E), the
+        breakpoint records of the weight path from 0 to 1 (DESIGN.md section 2g), the stop code, every point on the
+        path (column 0, row labels and the record count before it) and the end state.  The device tableau is restored
+        before the call returns."""
+        H, W = self.height, self.width
+        c2 = np.ascontiguousarray(cost2_by_label, dtype=np.float64)
+        if len(c2) != self.nVars:
+            raise ValueError(f"frontier: the objective has {len(c2)} entries, the tableau {self.nVars} labels")
+        # room for a point per breakpoint: np.empty only reserves address space, and the library writes the points
+        # the path has; beyond 1 GiB a longer path runs again with room for all of them
+        cap = min(max_breaks + 1, max(1, (1 << 30) // (12 * H))) if max_points is None else int(max_points)
+        while True:
+            r2, dirn = np.empty(W, dtype=np.float64), np.empty(W, dtype=np.float64)
+            theta, obj, dobj = (np.empty(max_breaks, dtype=np.float64) for _ in range(3))
+            rc = np.empty((max_breaks, 4), dtype=np.int32)
+            pt_rhs, pt_vrow = np.empty((max(1, cap), H), dtype=np.float64), np.empty((max(1, cap), H), dtype=np.int32)
+            pt_at = np.empty(max(1, cap), dtype=np.int32)
+            end_rhs, end_vrow = np.empty(H, dtype=np.float64), np.empty(H, dtype=np.int32)
+            n, stop, npts = C.c_int(), C.c_int(), C.c_int()
+            _lib.check(self.context.lib.jslp_frontier(
+                self._h(), c2.ctypes.data, int(max_breaks), int(cap), r2.ctypes.data, dirn.ctypes.data,
+                theta.ctypes.data, obj.ctypes.data, dobj.ctypes.data, rc.ctypes.data, C.byref(n), C.byref(stop),
+                pt_rhs.ctypes.data, pt_vrow.ctypes.data, pt_at.ctypes.data, C.byref(npts), end_rhs.ctypes.data,
+                end_vrow.ctypes.data))
+            if npts.value <= cap or max_points is not None:
+                break
+            cap = npts.value  # the path is deterministic: run it again with room for every point
+        k, p = n.value, min(npts.value, cap)
+        return {"r2": r2, "dir": dirn, "theta": theta[:k], "obj_raw": obj[:k], "dobj": dobj[:k], "rc_lbl": rc[:k],
+                "stop": stop.value, "pt_rhs": pt_rhs[:p], "pt_vrow": pt_vrow[:p], "pt_break": pt_at[:p],
+                "n_points": npts.value, "end_rhs": end_rhs, "end_vrow": end_vrow}
+
     def scenario_batch(self, edits, offsets, check_cycles: Optional[bool] = None) -> dict:
         """jslp_scenario_batch: edits = [(kind, index, difference), ...] with kind 0 = updateRightHandSide and 1 =
         updateCost; scenario s = edits[offsets[s]:offsets[s + 1]] applied to the current tableau, then simplex() (the
