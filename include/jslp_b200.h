@@ -273,6 +273,18 @@ int jslp_frontier(jslp_tab *tab, const double *cost2_by_label, int max_breaks, i
                   double *pt_rhs, int32_t *pt_vrow, int32_t *pt_break, int *n_points, double *end_rhs,
                   int32_t *end_vrow);
 
+/* The optimal face of the current (optimal) tableau as a sibling tab in the same context, DESIGN.md section 2h: column
+ * 0 and every column c >= 1 whose cost entry lies within the precision (M[0,c] >= -P && M[0,c] <= P) are kept, in
+ * order; the face holds rows 1.. of those columns bit for bit under a cost row of +0, the row labels, the kept column
+ * labels, and the parent's precision, unrestricted / integer tables, element indices and options.  Every vertex of the
+ * face is an optimum of the parent, so any objective set on it with jslp_update_cost / jslp_scenario_batch is
+ * optimised over the parent's optimal solutions.
+ *   face       the new tab (free it with jslp_tab_destroy); NULL when only column 0 is kept (n_keep = 1)
+ *   n_keep     kept columns W', column 0 included
+ *   kept_cols  NULL, or room for width entries: the first n_keep receive the kept columns of the parent
+ * The copy runs device to device; the parent is only read.  No optional objectives (JSLP_E_UNSUPPORTED). */
+int jslp_face_create(jslp_tab *tab, jslp_tab **face, int32_t *n_keep, int32_t *kept_cols);
+
 /* Multi-GPU communicator of the branch-and-cut frontier (one process per GPU).  NCCL is loaded at run time;
  * without libnccl these calls fail with JSLP_E_UNSUPPORTED and single-GPU use is unaffected.  Rank 0 obtains a
  * 128-byte unique id and hands it to the other ranks through whatever bootstrap the host has (the N-API host:

@@ -1373,3 +1373,4 @@ extern "C" int jslp_pivot_log(jslp_tab *t, int32_t *entries, int cap, int *n) {
 #include "jslp_scenario.cuh"
 #include "jslp_crash.cuh"
 #include "jslp_frontier.cuh"
+#include "jslp_face.cuh"

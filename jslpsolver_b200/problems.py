@@ -90,6 +90,36 @@ def dense_packing_lp_model(n_vars: int, n_cons: int, seed: int = 12345) -> dict:
             "constraints": constraints, "variables": variables}
 
 
+def alternative_optima_arrays(n_vars: int, n_cons: int, seed: int = 12345, dup: int = 3, par: int = 3):
+    """(A, b, c) of a packing LP `max c.x, A x <= b, x >= 0` whose optimum is not unique (dual degeneracy planted two
+    ways).  The first n_vars - dup - par columns and n_cons - 1 rows are dense_packing_lp_arrays' distributions, with
+    the costs of the first `dup` columns raised by 50 so that they tend to be basic; the next `dup` columns repeat
+    those columns and costs exactly (a copy of a basic variable has reduced cost 0).  The last `par` variables appear
+    only in the last row, `blend`, with entries a_j ~ U{1..20} and costs exactly 3 a_j: the objective is parallel to
+    that row over them, the row binds, and all but one of them are non-basic at reduced cost 0."""
+    base = n_vars - dup - par
+    assert dup >= 0 and par >= 0 and base >= dup and n_cons >= 2
+    rng = np.random.default_rng(seed)
+    A = np.zeros((n_cons, n_vars), dtype=np.float64)
+    A[:n_cons - 1, :base] = rng.integers(1, 21, size=(n_cons - 1, base))
+    b = rng.integers(100, 501, size=n_cons).astype(np.float64)
+    c = np.zeros(n_vars, dtype=np.float64)
+    c[:base] = rng.integers(1, 51, size=base)
+    c[:dup] += 50.0
+    A[:, base:base + dup] = A[:, :dup]
+    c[base:base + dup] = c[:dup]
+    A[n_cons - 1, base + dup:] = rng.integers(1, 21, size=par)
+    c[base + dup:] = 3.0 * A[n_cons - 1, base + dup:]
+    return A, b, c
+
+
+def alternative_optima_model(n_vars: int, n_cons: int, seed: int = 12345, dup: int = 3, par: int = 3) -> dict:
+    """alternative_optima_arrays as a jsLPSolver JSON model (lp_model's names: x0.., c0..)."""
+    m = lp_model(*alternative_optima_arrays(n_vars, n_cons, seed, dup, par))
+    m["name"] = f"AlternativeOptima_{n_vars}x{n_cons}_seed{seed}"
+    return m
+
+
 def dense_packing_multi_model(n_vars: int, n_cons: int, n_objectives: int, seed: int = 12345) -> dict:
     """dense_packing_lp_model with `optimize` = {profit: max, attr1: max, ...}: the extra objective attributes are
     U{1..50} per variable, drawn from the same seed after the packing instance."""

@@ -125,6 +125,20 @@ class Solution:  # solution.ts:16-61
         from .scenarios import compute
         return compute(self, cases)
 
+    def variability(self, variables=None, constraints=None, points=False) -> dict:
+        """Alternative optima of this continuous LP (DESIGN.md section 2h): over all optimal solutions, the range of
+        every structural variable, {"value", "min", "max", "fixed"} under "variables", and of every row's slack,
+        {"name", "type", "slack": {"value", "min", "max"}} under "constraints" in tableau order (an equality or a
+        min+max constraint is two rows).  Ends are raw doubles, +-inf where the optimal face is unbounded, None where
+        the LP behind an end gave no answer ("exact" is then False).  "unique" says whether every structural variable
+        of the model moves by no more than the precision; it covers all of them even when variables= (a list of ids)
+        or constraints= (a list of names) restricts what is reported.  points=True adds "argmin" / "argmax", the
+        optimal vertex {id: value} where each end is reached.  "free" counts the non-basic columns at reduced cost 0,
+        "lps" the LPs solved.  The tableau and the model are left unchanged; raises ValueError where sensitivity()
+        does, for unknown names and for models with unrestricted variables."""
+        from .variability import compute
+        return compute(self, variables=variables, constraints=constraints, points=points)
+
     def generateSolutionSet(self) -> dict:
         t = self._tableau
         if t.handle is None:
@@ -701,6 +715,26 @@ class GpuTableau:
             self._h(), arr, off.ctypes.data, n, cc, status.ctypes.data, eval_raw.ctypes.data, p1.ctypes.data,
             p2.ctypes.data, rhs.ctypes.data, vrow.ctypes.data))
         return {"status": status, "eval_raw": eval_raw, "p1": p1, "p2": p2, "rhs": rhs, "vrow": vrow}
+
+    def face(self):
+        """jslp_face_create: (face, kept columns).  `face` is a GpuTableau of the optimal face of the current (optimal)
+        tableau -- the columns whose cost entry lies within the precision, under a zero cost row, with this
+        tableau's row labels, options and model (DESIGN.md section 2h) -- or None when only column 0 is kept.  The
+        copy stays on the device; this tableau is only read.  close() the face when done."""
+        L = self.context.lib
+        h, n = C.c_void_p(), C.c_int32()
+        kept = np.empty(self.width, dtype=np.int32)
+        _lib.check(L.jslp_face_create(self._h(), C.byref(h), C.byref(n), kept.ctypes.data))
+        kept = kept[:n.value].copy()
+        if not h.value:
+            return None, kept
+        f = GpuTableau(self.precision, context=self.context)
+        f.handle = h
+        f.model, f.variablesPerIndex = self.model, self.variablesPerIndex
+        f.width, f.height = n.value, self.height
+        f.nVars, f.lastElementIndex, f.nOpt, f.nInts = self.nVars, self.lastElementIndex, 0, getattr(self, "nInts", 0)
+        f.engine, f.options = self.engine, dict(self.options)
+        return f, kept
 
     def crash(self, enter, leave):
         """jslp_crash: pivot the labels `enter` into the basis in order, each on the row with the largest |entry| among
