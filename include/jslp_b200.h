@@ -285,6 +285,18 @@ int jslp_frontier(jslp_tab *tab, const double *cost2_by_label, int max_breaks, i
  * The copy runs device to device; the parent is only read.  No optional objectives (JSLP_E_UNSUPPORTED). */
 int jslp_face_create(jslp_tab *tab, jslp_tab **face, int32_t *n_keep, int32_t *kept_cols);
 
+/* The current (optimal) tableau with its objective turned into a bound row, as a sibling tab in the same context,
+ * DESIGN.md section 2i: with M the tableau (H x W) and l* = max(n_index, lastElementIndex), the new tab B is (H+1) x W
+ * with the same stride; rows 1..H-1 are M's rows bit for bit, row 0 is +0 everywhere, and row H is B[H,0] = allowance,
+ * B[H,c] = -M[0,c] (a sign flip) for c >= 1.  Its row labels are M's followed by l*, its column labels M's; precision,
+ * unrestricted / integer tables (l* restricted, not integer), element indices and options are the parent's, with
+ * lastElementIndex = l* + 1.  Every feasible point of B is a point of the parent at most `allowance` worse than the
+ * optimum, so any objective set on it with jslp_update_cost / jslp_scenario_batch is optimised over those points.
+ *   allowance  finite and >= 0 (JSLP_E_INVALID otherwise)
+ *   bound      the new tab (free it with jslp_tab_destroy)
+ * The copy runs device to device; the parent is only read.  No optional objectives (JSLP_E_UNSUPPORTED). */
+int jslp_bound_create(jslp_tab *tab, double allowance, jslp_tab **bound);
+
 /* Multi-GPU communicator of the branch-and-cut frontier (one process per GPU).  NCCL is loaded at run time;
  * without libnccl these calls fail with JSLP_E_UNSUPPORTED and single-GPU use is unaffected.  Rank 0 obtains a
  * 128-byte unique id and hands it to the other ranks through whatever bootstrap the host has (the N-API host:

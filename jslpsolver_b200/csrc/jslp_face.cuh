@@ -98,6 +98,34 @@ __global__ void __launch_bounds__(FACE_TILE * FACE_TILE) k_face_gather(const Tab
 
 }  // namespace jslp
 
+// What a sibling tab (jslp_face_create, jslp_bound_create) takes over from its parent besides the tableau: the
+// unrestricted / integer tables over labels [0, n_index) and every jslp_tab_set_option value.  n_index >= the
+// parent's; the labels from the parent's n_index on are restricted and not integer.  The element indices stay the
+// parent's, so a label means the same in both tabs.
+static int inherit_tables_and_options(const jslp_tab *t, jslp_tab *f, int n_index) {
+    cudaStream_t s = t->ctx->stream;
+    const size_t n0 = (size_t)t->n_index, n1 = (size_t)n_index;
+    f->n_index = n_index;
+    if (t->hd.unres) {
+        CK(cudaMalloc(&f->hd.unres, n1));
+        if (n1 > n0) CK(cudaMemsetAsync(f->hd.unres + n0, 0, n1 - n0, s));
+        CK(cudaMemcpyAsync(f->hd.unres, t->hd.unres, n0, cudaMemcpyDeviceToDevice, s));
+    }
+    if (t->hd.intpos) {
+        CK(cudaMalloc(&f->hd.intpos, sizeof(int) * n1));
+        if (n1 > n0) CK(cudaMemsetAsync(f->hd.intpos + n0, 0xff, sizeof(int) * (n1 - n0), s));
+        CK(cudaMemcpyAsync(f->hd.intpos, t->hd.intpos, sizeof(int) * n0, cudaMemcpyDeviceToDevice, s));
+    }
+    f->h_intpos = t->h_intpos; f->n_int = t->n_int;
+    if (!f->h_intpos.empty() && f->h_intpos.size() < n1) f->h_intpos.resize(n1, -1);
+    f->engine = t->engine; f->batch = t->batch; f->host_log_cap = t->host_log_cap;
+    f->variant = t->variant; f->grid_per_sm = t->grid_per_sm; f->lookahead = t->lookahead;
+    f->timeline_cap = t->timeline_cap; f->pdl = t->pdl; f->pingpong = t->pingpong;
+    f->node_slots = t->node_slots; f->node_log_cap = t->node_log_cap; f->slot_steps = t->slot_steps;
+    f->slot_variant = t->slot_variant; f->use_mir = t->use_mir;
+    return JSLP_OK;
+}
+
 extern "C" int jslp_face_create(jslp_tab *t, jslp_tab **face, int32_t *n_keep, int32_t *kept_cols) {
     if (!t || !face || !n_keep) return fail(JSLP_E_INVALID, "NULL argument");
     *face = nullptr;
@@ -127,22 +155,10 @@ extern "C" int jslp_face_create(jslp_tab *t, jslp_tab **face, int32_t *n_keep, i
         if (Wk == 1) return JSLP_OK;  // nothing but column 0: the optimum is the only point of the face
         int rc2 = jslp_tab_create(ctx, Wk, H, t->rowcap, t->precision, &f);
         if (rc2) return rc2;
-        // labels, tables and options of the parent; the element indices stay the parent's, so labels mean the same
-        f->n_index = t->n_index; f->nVars = t->nVars; f->lastElementIndex = t->lastElementIndex;
-        if (t->hd.unres) {
-            CK(cudaMalloc(&f->hd.unres, (size_t)t->n_index));
-            CK(cudaMemcpyAsync(f->hd.unres, t->hd.unres, (size_t)t->n_index, cudaMemcpyDeviceToDevice, s));
-        }
-        if (t->hd.intpos) {
-            CK(cudaMalloc(&f->hd.intpos, sizeof(int) * (size_t)t->n_index));
-            CK(cudaMemcpyAsync(f->hd.intpos, t->hd.intpos, sizeof(int) * (size_t)t->n_index, cudaMemcpyDeviceToDevice, s));
-        }
-        f->h_intpos = t->h_intpos; f->n_int = t->n_int;
-        f->engine = t->engine; f->batch = t->batch; f->host_log_cap = t->host_log_cap;
-        f->variant = t->variant; f->grid_per_sm = t->grid_per_sm; f->lookahead = t->lookahead;
-        f->timeline_cap = t->timeline_cap; f->pdl = t->pdl; f->pingpong = t->pingpong;
-        f->node_slots = t->node_slots; f->node_log_cap = t->node_log_cap; f->slot_steps = t->slot_steps;
-        f->slot_variant = t->slot_variant; f->use_mir = t->use_mir;
+        // labels, tables and options of the parent
+        f->nVars = t->nVars; f->lastElementIndex = t->lastElementIndex;
+        rc2 = inherit_tables_and_options(t, f, t->n_index);
+        if (rc2) return rc2;
         rc2 = push_desc(f);
         if (rc2) return rc2;
         CK(cudaMemcpyAsync(f->hd.vcol, d_vcol, sizeof(int) * (size_t)Wk, cudaMemcpyDeviceToDevice, s));

@@ -125,7 +125,7 @@ class Solution:  # solution.ts:16-61
         from .scenarios import compute
         return compute(self, cases)
 
-    def variability(self, variables=None, constraints=None, points=False) -> dict:
+    def variability(self, variables=None, constraints=None, points=False, *, gap=0.0, absolute_gap=0.0) -> dict:
         """Alternative optima of this continuous LP (DESIGN.md section 2h): over all optimal solutions, the range of
         every structural variable, {"value", "min", "max", "fixed"} under "variables", and of every row's slack,
         {"name", "type", "slack": {"value", "min", "max"}} under "constraints" in tableau order (an equality or a
@@ -135,9 +135,15 @@ class Solution:  # solution.ts:16-61
         or constraints= (a list of names) restricts what is reported.  points=True adds "argmin" / "argmax", the
         optimal vertex {id: value} where each end is reached.  "free" counts the non-basic columns at reduced cost 0,
         "lps" the LPs solved.  The tableau and the model are left unchanged; raises ValueError where sensitivity()
-        does, for unknown names and for models with unrestricted variables."""
+        does, for unknown names and for models with unrestricted variables.
+
+        Near-optimal variability (DESIGN.md section 2i): with an allowance t = max(absolute_gap, gap * |result|) > 0,
+        the ranges are taken over every feasible plan whose objective is at most t worse than the optimum instead, no
+        column is banned ("free" counts every non-basic column), and the report gains "allowance": t.  t == 0, the
+        default, is exactly the report above.  gap= and absolute_gap= must be finite numbers >= 0."""
         from .variability import compute
-        return compute(self, variables=variables, constraints=constraints, points=points)
+        return compute(self, variables=variables, constraints=constraints, points=points, gap=gap,
+                       absolute_gap=absolute_gap)
 
     def generateSolutionSet(self) -> dict:
         t = self._tableau
@@ -735,6 +741,23 @@ class GpuTableau:
         f.nVars, f.lastElementIndex, f.nOpt, f.nInts = self.nVars, self.lastElementIndex, 0, getattr(self, "nInts", 0)
         f.engine, f.options = self.engine, dict(self.options)
         return f, kept
+
+    def bound(self, allowance: float) -> "GpuTableau":
+        """jslp_bound_create: a GpuTableau of the current (optimal) tableau with its objective turned into one bound
+        row -- the rows below the cost row unchanged, a zero cost row, and a last row whose slack is `allowance` minus
+        the objective a point gives up against the optimum -- with this tableau's column labels, options and model
+        and one new row label, max(nVars, lastElementIndex) (DESIGN.md section 2i).  The copy stays on the device;
+        this tableau is only read.  close() the bound tableau when done."""
+        L = self.context.lib
+        h = C.c_void_p()
+        _lib.check(L.jslp_bound_create(self._h(), float(allowance), C.byref(h)))
+        b = GpuTableau(self.precision, context=self.context)
+        b.handle = h
+        b.model, b.variablesPerIndex = self.model, self.variablesPerIndex
+        b.nOpt, b.nInts = 0, getattr(self, "nInts", 0)
+        b.engine, b.options = self.engine, dict(self.options)
+        b._refresh_dims()
+        return b
 
     def crash(self, enter, leave):
         """jslp_crash: pivot the labels `enter` into the basis in order, each on the row with the largest |entry| among

@@ -7,15 +7,30 @@ With every reduced cost of the right sign, a feasible point is optimal exactly w
 non-zero reduced cost stays at 0.  The library gathers the other columns into a face tableau on the device
 (jslp_face_create) with a zero cost row; minimising and maximising one variable over it is the one-edit cost scenario
 of section 2e, and all of them run as one jslp_scenario_batch on the face, each warm-started from the optimal basis.
-This module resolves names, leaves out the LPs whose answer the tableau already shows, and shapes the result."""
+This module resolves names, leaves out the LPs whose answer the tableau already shows, and shapes the result.
+
+With gap= / absolute_gap= the ranges are taken over the plans whose objective is at most an allowance t worse than
+the optimum (DESIGN.md section 2i): instead of the face, the device builds the optimal tableau with its objective
+turned into one bound row (jslp_bound_create), bans no column, and runs the same target LPs on it."""
 from __future__ import annotations
 
 import math
+import numbers
 
 from .sensitivity import _check
 
 WHAT = "variability()"
 OPTIMAL, UNBOUNDED = 0, 2
+
+
+def _gap(name: str, x) -> float:
+    """A gap= / absolute_gap= argument as a float: a finite, non-negative number."""
+    if isinstance(x, bool) or not isinstance(x, numbers.Real):
+        raise ValueError(f"{WHAT}: {name}= takes a number, not {type(x).__name__}")
+    x = float(x)
+    if not (math.isfinite(x) and x >= 0.0):
+        raise ValueError(f"{WHAT}: {name}= must be finite and >= 0, not {x!r}")
+    return x
 
 
 def _end(status: int, eval_raw: float, sense: int):
@@ -34,9 +49,10 @@ def _point(m, fixed, rhs, vrow) -> dict:
             for v in m.variables}
 
 
-def compute(solution, variables=None, constraints=None, points=False) -> dict:
+def compute(solution, variables=None, constraints=None, points=False, gap=0.0, absolute_gap=0.0) -> dict:
     """Solution.variability(): see the module docstring."""
     _check(solution, WHAT)
+    gap, absolute_gap = _gap("gap", gap), _gap("absolute_gap", absolute_gap)
     t = solution._tableau
     m = t.model
     if any(m.unrestrictedVariables.values()):
@@ -64,8 +80,15 @@ def compute(solution, variables=None, constraints=None, points=False) -> dict:
         rows = [c for c in m.constraints if cname(c) in set(constraints)]
     fixed = m.presolveResult.fixedVariables if m.presolveResult is not None else {}
 
-    rhs, _, vrow, vcol = t.final_state()
-    face, kept = t.face()
+    rhs, cost, vrow, vcol = t.final_state()
+    # the allowance t = max(absolute_gap, gap * |z|), z = -sigma * M[0,0] the solved result (section 2i)
+    allowance = max(absolute_gap, gap * abs(float(cost[0])))
+    if math.isinf(allowance):
+        raise ValueError(f"{WHAT}: the allowance gap * |result| overflows (gap={gap!r}, result={-float(cost[0])!r})")
+    if allowance > 0.0:
+        face, kept = t.bound(allowance), range(len(vcol))  # the bound row bans no column
+    else:
+        face, kept = t.face()
     kept = {int(c) for c in kept}
     row_of = {int(vrow[r]): r for r in range(1, len(vrow))}
     col_of = {int(vcol[c]): c for c in range(1, len(vcol))}
@@ -124,5 +147,8 @@ def compute(solution, variables=None, constraints=None, points=False) -> dict:
     out_c = [{"name": cname(c), "type": "max" if c.isUpperBound else "min", "slack": shaped(entry[c.index], {})}
              for c in rows]
     exact = all(e["min"] is not None and e["max"] is not None for e in entry.values())
-    return {"unique": all(spread(v) <= t.precision for v in m.variables), "exact": exact, "variables": out_v,
-            "constraints": out_c, "free": len(kept) - 1, "lps": len(targets)}
+    report = {"unique": all(spread(v) <= t.precision for v in m.variables), "exact": exact, "variables": out_v,
+              "constraints": out_c, "free": len(kept) - 1, "lps": len(targets)}
+    if allowance > 0.0:
+        report["allowance"] = allowance
+    return report
