@@ -297,6 +297,22 @@ int jslp_face_create(jslp_tab *tab, jslp_tab **face, int32_t *n_keep, int32_t *k
  * The copy runs device to device; the parent is only read.  No optional objectives (JSLP_E_UNSUPPORTED). */
 int jslp_bound_create(jslp_tab *tab, double allowance, jslp_tab **bound);
 
+/* One step of a lexicographic objective chain, DESIGN.md section 2j: the starting tableau of the next level from the
+ * current (optimal) tableau, as a sibling tab in the same context.  With allowance == 0 it is jslp_face_create's face,
+ * with allowance > 0 jslp_bound_create's bound tableau; in both, row 0 is the next objective priced against the
+ * current basis instead of +0 -- R[c] = delta(c) + the section 2g block sums of -C[vrow[r]] * M[r,c] (jslp_frontier's
+ * r2), taken at the kept columns of a face and at every column of a bound tableau, padding +0.  Every other element,
+ * label, table and option is the face's or the bound tableau's.  Column 0 is the parent's (plus the allowance), so
+ * the new tab starts primal feasible and jslp_simplex runs phase 2 only.
+ *   cost_by_label  the next objective's row-0 entries by label (sigma * c_j at structural labels, 0 elsewhere), one
+ *                  per label of tab (nVars of jslp_tab_info)
+ *   allowance      finite and >= 0 (JSLP_E_INVALID otherwise)
+ *   next           the new tab (free it with jslp_tab_destroy); NULL when a face keeps only column 0
+ *   n_keep         W' (the tab's width for a bound tableau);  kept_cols (optional, W entries) the kept columns
+ * The copy and row 0 stay on the device; the parent is only read.  No optional objectives (JSLP_E_UNSUPPORTED). */
+int jslp_lex_next(jslp_tab *tab, const double *cost_by_label, double allowance, jslp_tab **next, int32_t *n_keep,
+                  int32_t *kept_cols);
+
 /* Multi-GPU communicator of the branch-and-cut frontier (one process per GPU).  NCCL is loaded at run time;
  * without libnccl these calls fail with JSLP_E_UNSUPPORTED and single-GPU use is unaffected.  Rank 0 obtains a
  * 128-byte unique id and hands it to the other ranks through whatever bootstrap the host has (the N-API host:

@@ -1375,3 +1375,4 @@ extern "C" int jslp_pivot_log(jslp_tab *t, int32_t *entries, int cap, int *n) {
 #include "jslp_frontier.cuh"
 #include "jslp_face.cuh"
 #include "jslp_bound.cuh"
+#include "jslp_lex.cuh"

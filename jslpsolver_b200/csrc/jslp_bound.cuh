@@ -39,12 +39,9 @@ __global__ void __launch_bounds__(BOUND_THREADS) k_bound_rows(const TabDev *Tp, 
 
 }  // namespace jslp
 
-extern "C" int jslp_bound_create(jslp_tab *t, double allowance, jslp_tab **out) {
-    if (!t || !out) return fail(JSLP_E_INVALID, "NULL argument");
-    *out = nullptr;
-    if (!(allowance >= 0.0) || std::isinf(allowance))
-        return fail(JSLP_E_INVALID, "bound_create: the allowance must be finite and >= 0");
-    if (t->nOpt > 0) return fail(JSLP_E_UNSUPPORTED, "bound_create: optional objectives are not supported");
+// The bound tableau of t into *out.  With d_cost (a device array of C by label) row 0 is the next objective priced
+// against t at every column (k_price_objective, section 2j) instead of +0.
+static int bound_build(jslp_tab *t, double allowance, const double *d_cost, jslp_tab **out) {
     jslp_ctx *ctx = t->ctx;
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = ctx->stream;
@@ -78,6 +75,12 @@ extern "C" int jslp_bound_create(jslp_tab *t, double allowance, jslp_tab **out) 
                                                                                               b->stride, b->hd.vrow, label);
         ctx->launches += 1;
         CK(cudaGetLastError());
+        if (d_cost) {  // over the +0 k_bound_rows wrote at columns 0..W-1; the padding stays +0
+            k_price_objective<<<(W + FR_COLS - 1) / FR_COLS, FR_COLS, 0, s>>>(t->d_T, d_cost, nullptr, W, b->hd.M,
+                                                                              nullptr);
+            ctx->launches += 1;
+            CK(cudaGetLastError());
+        }
         CK(cudaStreamSynchronize(s));
         return JSLP_OK;
     };
@@ -88,4 +91,13 @@ extern "C" int jslp_bound_create(jslp_tab *t, double allowance, jslp_tab **out) 
     }
     *out = b;
     return JSLP_OK;
+}
+
+extern "C" int jslp_bound_create(jslp_tab *t, double allowance, jslp_tab **out) {
+    if (!t || !out) return fail(JSLP_E_INVALID, "NULL argument");
+    *out = nullptr;
+    if (!(allowance >= 0.0) || std::isinf(allowance))
+        return fail(JSLP_E_INVALID, "bound_create: the allowance must be finite and >= 0");
+    if (t->nOpt > 0) return fail(JSLP_E_UNSUPPORTED, "bound_create: optional objectives are not supported");
+    return bound_build(t, allowance, nullptr, out);
 }

@@ -126,10 +126,9 @@ static int inherit_tables_and_options(const jslp_tab *t, jslp_tab *f, int n_inde
     return JSLP_OK;
 }
 
-extern "C" int jslp_face_create(jslp_tab *t, jslp_tab **face, int32_t *n_keep, int32_t *kept_cols) {
-    if (!t || !face || !n_keep) return fail(JSLP_E_INVALID, "NULL argument");
-    *face = nullptr;
-    if (t->nOpt > 0) return fail(JSLP_E_UNSUPPORTED, "face_create: optional objectives are not supported");
+// The face of t into *face (nullptr when only column 0 is kept).  With d_cost (a device array of C by label) row 0 is
+// the next objective priced against t at the kept columns (k_price_objective through map[], section 2j) instead of +0.
+static int face_build(jslp_tab *t, const double *d_cost, jslp_tab **face, int32_t *n_keep, int32_t *kept_cols) {
     jslp_ctx *ctx = t->ctx;
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = ctx->stream;
@@ -166,6 +165,12 @@ extern "C" int jslp_face_create(jslp_tab *t, jslp_tab **face, int32_t *n_keep, i
         k_face_gather<<<grid, FACE_TILE * FACE_TILE, 0, s>>>(t->d_T, d_map, Wk, f->hd.M, f->stride, f->hd.vrow);
         ctx->launches += 1;
         CK(cudaGetLastError());
+        if (d_cost) {  // over the +0 the gather wrote at the kept columns; the padding stays +0
+            k_price_objective<<<(Wk + FR_COLS - 1) / FR_COLS, FR_COLS, 0, s>>>(t->d_T, d_cost, d_map, Wk, f->hd.M,
+                                                                               nullptr);
+            ctx->launches += 1;
+            CK(cudaGetLastError());
+        }
         CK(cudaStreamSynchronize(s));
         return JSLP_OK;
     };
@@ -177,4 +182,11 @@ extern "C" int jslp_face_create(jslp_tab *t, jslp_tab **face, int32_t *n_keep, i
     }
     *face = f;
     return JSLP_OK;
+}
+
+extern "C" int jslp_face_create(jslp_tab *t, jslp_tab **face, int32_t *n_keep, int32_t *kept_cols) {
+    if (!t || !face || !n_keep) return fail(JSLP_E_INVALID, "NULL argument");
+    *face = nullptr;
+    if (t->nOpt > 0) return fail(JSLP_E_UNSUPPORTED, "face_create: optional objectives are not supported");
+    return face_build(t, nullptr, face, n_keep, kept_cols);
 }

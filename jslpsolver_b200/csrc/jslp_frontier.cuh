@@ -17,10 +17,13 @@ namespace jslp {
 static constexpr int FR_ROWS = 64;   // rows per block of the pricing sum (part of the contract: it fixes the order)
 static constexpr int FR_COLS = 128;  // columns per CTA of k_price_objective, one per thread
 
-// R2 and E of section 2g.  One CTA per FR_COLS columns walks every row block in order; two warps compact the block's
+// R2 and E of section 2g.  One CTA per FR_COLS outputs walks every row block in order; two warps compact the block's
 // rows with a non-zero coefficient (ascending) into shared memory, then every thread runs its column's partial over
-// them.  The grid only splits columns, so any grid gives the same bits.
-__global__ void __launch_bounds__(FR_COLS) k_price_objective(const TabDev *Tp, const double *c2, double *r2, double *e) {
+// them.  The grid only splits columns, so any grid gives the same bits.  Output k < n_out is column c = map[k] (c = k
+// without a map) and goes to r2[k] and, when e is given, e[k]; jslp_frontier prices every column (no map, n_out = W),
+// jslp_lex_next writes R straight into row 0 of the next level's tableau, through the face's kept-column map.
+__global__ void __launch_bounds__(FR_COLS) k_price_objective(const TabDev *Tp, const double *c2, const int *map,
+                                                             int n_out, double *r2, double *e) {
     __shared__ TabDev T;
     __shared__ int s_row[FR_ROWS];
     __shared__ double s_coef[FR_ROWS];
@@ -28,10 +31,11 @@ __global__ void __launch_bounds__(FR_COLS) k_price_objective(const TabDev *Tp, c
     const int tid = threadIdx.x;
     if (tid == 0) T = *Tp;
     __syncthreads();
-    const int H = T.H, W = T.W;
+    const int H = T.H;
     const size_t stride = (size_t)T.stride;
-    const int c = blockIdx.x * FR_COLS + tid;
-    const bool in = c < W;
+    const int k_out = blockIdx.x * FR_COLS + tid;
+    const bool in = k_out < n_out;
+    const int c = in && map ? map[k_out] : k_out;
     double R = 0.0;
     if (in && c > 0) R = c2[T.vcol[c]];
     for (int r0 = 1; r0 < H; r0 += FR_ROWS) {
@@ -63,8 +67,8 @@ __global__ void __launch_bounds__(FR_COLS) k_price_objective(const TabDev *Tp, c
         __syncthreads();  // the lists are rewritten by the next block
     }
     if (in) {
-        r2[c] = R;
-        e[c] = __dsub_rn(R, ldg_cg(T.M + c));
+        r2[k_out] = R;
+        if (e) e[k_out] = __dsub_rn(R, ldg_cg(T.M + c));
     }
 }
 
@@ -159,7 +163,7 @@ extern "C" int jslp_frontier(jslp_tab *t, const double *cost2_by_label, int max_
     if (rc) return rc;
     CK(cudaMemcpyAsync(b.c2, cost2_by_label, sizeof(double) * (size_t)t->n_index, cudaMemcpyHostToDevice, s));
     CK(cudaMemsetAsync(b.e, 0, sizeof(double) * (size_t)t->stride, s));
-    k_price_objective<<<(t->W + FR_COLS - 1) / FR_COLS, FR_COLS, 0, s>>>(t->d_T, b.c2, b.r2, b.e);
+    k_price_objective<<<(t->W + FR_COLS - 1) / FR_COLS, FR_COLS, 0, s>>>(t->d_T, b.c2, nullptr, t->W, b.r2, b.e);
     t->ctx->launches += 1;
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(r2, b.r2, sizeof(double) * (size_t)t->W, cudaMemcpyDeviceToHost, s));

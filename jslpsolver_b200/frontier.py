@@ -27,13 +27,13 @@ def _objectives(model: dict):
     return keys, {k: "max" if opt[k] == "max" else "min" for k in keys}
 
 
-def _refuse(model: dict) -> None:
+def _refuse(model: dict, what: str = WHAT) -> None:
     if any(_truthy(v) for v in (model.get("ints") or {}).values()) or \
             any(_truthy(v) for v in (model.get("binaries") or {}).values()):
-        raise ValueError(f"{WHAT} is defined for continuous LPs only: the model has integer or binary variables")
+        raise ValueError(f"{what} is defined for continuous LPs only: the model has integer or binary variables")
     for spec in (model.get("constraints") or {}).values():
         if isinstance(spec, dict) and (spec.get("weight") is not None or spec.get("priority") is not None):
-            raise ValueError(f"{WHAT} does not support soft constraints (weight / priority)")
+            raise ValueError(f"{what} does not support soft constraints (weight / priority)")
 
 
 def _coef(jm: dict, vid: str, key: str) -> float:
@@ -85,6 +85,17 @@ def vertices(points, starts, end, stop, precision):
     return [tuple(s) for s in out]
 
 
+def objective_sums(m, jm: dict, keys, pt) -> dict:
+    """{key: the sum of c_key,j * x_j in variable order} at the point pt (structural values in m.variables order)."""
+    objs = {}
+    for key in keys:
+        acc = 0.0
+        for v, x in zip(m.variables, pt):
+            acc += _coef(jm, v.id, key) * x
+        objs[key] = acc
+    return objs
+
+
 def result(m, jm: dict, keys, senses, out) -> dict:
     """The Frontier() result from a frontier_path() output on the tableau of model `m` (loaded from `jm`)."""
     fixed = m.presolveResult.fixedVariables if m.presolveResult is not None else {}
@@ -100,13 +111,8 @@ def result(m, jm: dict, keys, senses, out) -> dict:
     out_v = []
     for pt, lo, hi in vertices(points, starts, end, stop, m.precision):
         values = {v.id: x for v, x in zip(m.variables, pt)}
-        objs = {}
-        for key in keys:
-            acc = 0.0
-            for v, x in zip(m.variables, pt):
-                acc += _coef(jm, v.id, key) * x
-            objs[key] = acc
-        out_v.append({"weight": {"from": lo, "to": hi}, "objectives": objs, "values": values})
+        out_v.append({"weight": {"from": lo, "to": hi}, "objectives": objective_sums(m, jm, keys, pt),
+                      "values": values})
     pivots = sum(1 for r in out["rc_lbl"] if int(r[0]) >= 0 and int(r[1]) >= 0)
     return {"feasible": True, "objectives": dict(senses), "vertices": out_v, "stop": stop, "end": end,
             "pivots": pivots}

@@ -120,6 +120,25 @@ def alternative_optima_model(n_vars: int, n_cons: int, seed: int = 12345, dup: i
     return m
 
 
+def alternative_optima_multi_model(n_vars: int, n_cons: int, n_objectives: int, seed: int = 12345, dup: int = 3,
+                                   par: int = 3) -> dict:
+    """alternative_optima_model with `optimize` = {objective: max, obj1: min, obj2: max, ...} (the extra senses
+    alternate, starting with min).  The extra attributes are U{0..20} per variable from a generator seeded with (seed,
+    n_objectives); the `dup` copies take their originals' values, so every objective keeps each copy tied with its
+    original and a face at allowance 0 is not a single point."""
+    m = alternative_optima_model(n_vars, n_cons, seed, dup, par)
+    m["name"] = f"AlternativeOptima{n_objectives}obj_{n_vars}x{n_cons}_seed{seed}"
+    base = n_vars - dup - par
+    rng = np.random.default_rng((seed, n_objectives))
+    extra = rng.integers(0, 21, size=(n_objectives - 1, n_vars)).astype(np.float64)
+    extra[:, base:base + dup] = extra[:, :dup]
+    m["optimize"] = {"objective": "max", **{f"obj{k}": "min" if k % 2 else "max" for k in range(1, n_objectives)}}
+    for j, v in enumerate(m["variables"].values()):
+        for k in range(1, n_objectives):
+            v[f"obj{k}"] = float(extra[k - 1, j])
+    return m
+
+
 def dense_packing_multi_model(n_vars: int, n_cons: int, n_objectives: int, seed: int = 12345) -> dict:
     """dense_packing_lp_model with `optimize` = {profit: max, attr1: max, ...}: the extra objective attributes are
     U{1..50} per variable, drawn from the same seed after the packing instance."""

@@ -6,6 +6,7 @@ from typing import Any, Optional
 
 from . import validation
 from .frontier import Frontier as _frontier
+from .lexicographic import Lexicographic as _lexicographic
 from .model import Model, object_keys
 from .polyopt import Polyopt
 
@@ -63,6 +64,12 @@ class Solver:
         objective's optimum to the second's, with the weights that select it (frontier.py, DESIGN.md section 2g)."""
         return _frontier(self, model, precision, validate)
 
+    def Lexicographic(self, model: dict, gap=0.0, absolute_gap=0.0, precision: Optional[float] = None,
+                      validate: bool = False) -> dict:
+        """Hierarchical objectives of a continuous LP: the objectives of `optimize` in order, each optimised over the
+        plans within an allowance of every earlier optimum (lexicographic.py, DESIGN.md section 2j)."""
+        return _lexicographic(self, model, gap, absolute_gap, precision, validate)
+
     def _instance(self, model: Any, precision: Optional[float]) -> Model:
         if isinstance(model, dict):
             options = model.get("options") or {}
@@ -115,3 +122,8 @@ def Solve(model: Any, precision: Optional[float] = None, full: bool = False, val
 
 def Frontier(model: dict, precision: Optional[float] = None, validate: bool = False) -> dict:
     return solver.Frontier(model, precision, validate)
+
+
+def Lexicographic(model: dict, gap=0.0, absolute_gap=0.0, precision: Optional[float] = None,
+                  validate: bool = False) -> dict:
+    return solver.Lexicographic(model, gap, absolute_gap, precision, validate)

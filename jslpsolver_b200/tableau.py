@@ -289,9 +289,11 @@ class GpuTableau:
         self._edited()
 
     # ------------------------------------------------------------------ simplex (tableau.ts:103-123)
-    def simplex(self) -> "GpuTableau":
+    def simplex(self, check_cycles: Optional[bool] = None) -> "GpuTableau":
+        """jslp_simplex with the model's cycle check, unless check_cycles is given."""
         st = LpStatus()
-        _lib.check(self.context.lib.jslp_simplex(self._h(), self._check_cycles(), C.byref(st)))
+        cc = self._check_cycles() if check_cycles is None else int(bool(check_cycles))
+        _lib.check(self.context.lib.jslp_simplex(self._h(), cc, C.byref(st)))
         self._absorb(st)
         self._solved_version = self._version
         return self
@@ -758,6 +760,31 @@ class GpuTableau:
         b.engine, b.options = self.engine, dict(self.options)
         b._refresh_dims()
         return b
+
+    def lex_next(self, cost_by_label, allowance: float):
+        """jslp_lex_next: (next, kept columns).  `next` is the starting tableau of the next level of a lexicographic
+        chain (DESIGN.md section 2j): face() for allowance == 0, bound(allowance) for allowance > 0, with row 0 the
+        objective `cost_by_label` (one entry per label, nVars) priced against the current basis; None when a face
+        keeps only column 0.  The copy and row 0 stay on the device; this tableau is only read.  close() it when
+        done."""
+        c = np.ascontiguousarray(cost_by_label, dtype=np.float64)
+        if len(c) != self.nVars:
+            raise ValueError(f"lex_next: the objective has {len(c)} entries, the tableau {self.nVars} labels")
+        L = self.context.lib
+        h, n = C.c_void_p(), C.c_int32()
+        kept = np.empty(self.width, dtype=np.int32)
+        _lib.check(L.jslp_lex_next(self._h(), c.ctypes.data, float(allowance), C.byref(h), C.byref(n),
+                                   kept.ctypes.data))
+        kept = kept[:n.value].copy()
+        if not h.value:
+            return None, kept
+        f = GpuTableau(self.precision, context=self.context)
+        f.handle = h
+        f.model, f.variablesPerIndex = self.model, self.variablesPerIndex
+        f.nOpt, f.nInts = 0, getattr(self, "nInts", 0)
+        f.engine, f.options = self.engine, dict(self.options)
+        f._refresh_dims()
+        return f, kept
 
     def crash(self, enter, leave):
         """jslp_crash: pivot the labels `enter` into the basis in order, each on the row with the largest |entry| among

@@ -23,13 +23,13 @@ WHAT = "variability()"
 OPTIMAL, UNBOUNDED = 0, 2
 
 
-def _gap(name: str, x) -> float:
+def _gap(name: str, x, what: str = WHAT) -> float:
     """A gap= / absolute_gap= argument as a float: a finite, non-negative number."""
     if isinstance(x, bool) or not isinstance(x, numbers.Real):
-        raise ValueError(f"{WHAT}: {name}= takes a number, not {type(x).__name__}")
+        raise ValueError(f"{what}: {name}= takes a number, not {type(x).__name__}")
     x = float(x)
     if not (math.isfinite(x) and x >= 0.0):
-        raise ValueError(f"{WHAT}: {name}= must be finite and >= 0, not {x!r}")
+        raise ValueError(f"{what}: {name}= must be finite and >= 0, not {x!r}")
     return x
 
 
