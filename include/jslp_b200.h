@@ -313,6 +313,23 @@ int jslp_bound_create(jslp_tab *tab, double allowance, jslp_tab **bound);
 int jslp_lex_next(jslp_tab *tab, const double *cost_by_label, double allowance, jslp_tab **next, int32_t *n_keep,
                   int32_t *kept_cols);
 
+/* The elastic tableau of a possibly infeasible LP, DESIGN.md section 2k: a sibling tab in the same context in which
+ * the relaxable rows r_1 < ... < r_k each get a violation column e_j (>= 0, in the constraint's own units) and row 0
+ * is the weighted total violation sum_j w_j e_j.  With M the tab (H x W), P its precision and l* = max(n_index,
+ * lastElementIndex), the new tab E is H x (W + k): column W+j enters row r_j as -1 (s.a.x <= s.rhs + e_j); a row with
+ * M[r_j,0] < -P is crashed onto e_j (its entries sign-flipped, column 0 included; vrow[r_j] = l*+j and the slack's
+ * label moves to column W+j); every other element of rows 1..H-1 is M's bit for bit, elastic entries of other rows
+ * +0; row 0 is sum over crashed j of w_j * E[r_j,c] in the fixed order of section 2k, and -w_j at the elastic column
+ * of a row that is not crashed.  The new labels are restricted and not integer; tables and options are the parent's.
+ * Rows that start below -P may all be relaxed => E starts primal feasible and jslp_simplex runs phase 2 only.
+ *   rows, weights  k increasing rows in 1..H-1 whose basic label is still the one they were uploaded with (the tab
+ *                  as jslp_tab_upload left it), weights finite and > 0 (JSLP_E_INVALID otherwise)
+ *   elastic        the new tab (free it with jslp_tab_destroy); JSLP_E_CAPACITY when W + k is beyond the width cap
+ *   n_crashed      the number of crashed rows
+ * The parent is only read; nothing but the crash count leaves the device.  No optional objectives (JSLP_E_INVALID). */
+int jslp_elastic_create(jslp_tab *tab, const int32_t *rows, const double *weights, int n_rows, jslp_tab **elastic,
+                        int32_t *n_crashed);
+
 /* Multi-GPU communicator of the branch-and-cut frontier (one process per GPU).  NCCL is loaded at run time;
  * without libnccl these calls fail with JSLP_E_UNSUPPORTED and single-GPU use is unaffected.  Rank 0 obtains a
  * 128-byte unique id and hands it to the other ranks through whatever bootstrap the host has (the N-API host:

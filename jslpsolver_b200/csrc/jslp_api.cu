@@ -159,6 +159,7 @@ struct jslp_tab {
     NodeSlots slots;        // K3: HBM-resident node batch (jslp_slots.cuh)
     int use_mir = 0;        // model.useMIRCuts (JSLP_OPT_USE_MIR_CUTS)
     std::vector<int> h_intpos;  // host copy of TabDev.intpos (computeFractionalVolume runs on the host)
+    std::vector<int> h_vrow_upload;  // the row labels of the last jslp_tab_upload (jslp_elastic_create checks them)
     int *d_count = nullptr, *h_count = nullptr;
     int node_slots = -1;    // JSLP_OPT_NODE_SLOTS: -1 = auto, 0 = off (one node at a time), n = at most n slots
     int node_log_cap = 512; // pivot-log entries per node of the shared-memory node kernel (overflow -> HBM path)
@@ -372,6 +373,7 @@ extern "C" int jslp_tab_upload(jslp_tab *t, const double *matrix, const int32_t 
                          sizeof(double) * t->W, t->H, cudaMemcpyHostToDevice, s));
     CK(cudaMemcpyAsync(t->hd.vrow, vrow, sizeof(int) * t->H, cudaMemcpyHostToDevice, s));
     CK(cudaMemcpyAsync(t->hd.vcol, vcol, sizeof(int) * t->W, cudaMemcpyHostToDevice, s));
+    t->h_vrow_upload.assign(vrow, vrow + t->H);
     if (n_index > 0) t->n_index = n_index;
     cudaFree(t->hd.unres); t->hd.unres = nullptr;
     bool any_unres = false;
@@ -1376,3 +1378,4 @@ extern "C" int jslp_pivot_log(jslp_tab *t, int32_t *entries, int cap, int *n) {
 #include "jslp_face.cuh"
 #include "jslp_bound.cuh"
 #include "jslp_lex.cuh"
+#include "jslp_elastic.cuh"

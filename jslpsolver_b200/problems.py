@@ -206,6 +206,35 @@ def planted_infeasible_model(n_vars: int, n_cons: int, k: int, seed: int = 12345
             "constraints": constraints, "variables": variables}
 
 
+def infeasible_packing_arrays(n_vars: int, n_cons: int, n_demand: int, seed: int = 12345):
+    """(A, b, c, lower) of infeasible_packing_model: n_cons rows in all, of which n_demand (lower[i] True) are demand
+    rows at seeded positions in the row order and the others packing rows."""
+    assert 0 <= n_demand <= n_cons and n_vars >= 1
+    rng = np.random.default_rng(seed)
+    A = rng.integers(1, 21, size=(n_cons, n_vars)).astype(np.float64)
+    b = rng.integers(100, 501, size=n_cons).astype(np.float64)
+    c = rng.integers(1, 51, size=n_vars).astype(np.float64)
+    lower = np.zeros(n_cons, dtype=bool)
+    lower[rng.choice(n_cons, size=n_demand, replace=False)] = True
+    if n_demand < n_cons:
+        cap = float(b[~lower].min())
+        A[lower] = rng.integers(2, 5, size=(n_demand, n_vars)) / 4.0  # entries in {0.5, 0.75, 1}
+        b[lower] = cap + rng.integers(1, 21, size=n_demand)
+    return A, b, c, lower
+
+
+def infeasible_packing_model(n_vars: int, n_cons: int, n_demand: int, seed: int = 12345) -> dict:
+    """max c.x over a dense packing LP whose n_demand demand rows (`min`) make it infeasible by construction.  Packing
+    rows are a_i.x <= b_i with a_ij ~ U{1..20} and b_i ~ U{100..500}; a demand row is d.x >= cap + U{1..20} with d_j in
+    {0.5, 0.75, 1} and cap the smallest packing right-hand side.  Why no x >= 0 meets a demand row: every packing entry
+    is >= 1, so sum_j x_j <= a_i.x <= b_i for every packing row, hence sum_j x_j <= cap; every d_j <= 1, so d.x <=
+    sum_j x_j <= cap < the demand.  Each demand row starts below 0 in the tableau (it is stored negated), so they are
+    the rows a repair crashes.  n_cons counts all rows; with n_demand == n_cons there is no packing row and the model
+    is feasible."""
+    A, b, c, lower = infeasible_packing_arrays(n_vars, n_cons, n_demand, seed)
+    return dict(lp_model(A, b, c, lower), name=f"InfeasiblePacking_{n_vars}x{n_cons}_{n_demand}_seed{seed}")
+
+
 def knapsack_mip_model(n_items: int, n_cons: int, seed: int = 12345, tolerance: float = 0.0) -> dict:
     """Multi-dimensional 0/1 knapsack (SURVEY.md 8d config 5): a_ij ~ U{1..50} dense,
     b_i = floor(0.5 * sum_j a_ij), c_j ~ U{1..50}; every binary adds an `x <= 1` row

@@ -9,6 +9,7 @@ from .frontier import Frontier as _frontier
 from .lexicographic import Lexicographic as _lexicographic
 from .model import Model, object_keys
 from .polyopt import Polyopt
+from .repair import Repair as _repair
 
 
 class Solver:
@@ -70,6 +71,13 @@ class Solver:
         plans within an allowance of every earlier optimum (lexicographic.py, DESIGN.md section 2j)."""
         return _lexicographic(self, model, gap, absolute_gap, precision, validate)
 
+    def Repair(self, model: dict, weights=None, *, objective: bool = True, gap=0.0, absolute_gap=0.0,
+               precision: Optional[float] = None, validate: bool = False) -> dict:
+        """The least weighted relaxation of the rows of a (possibly infeasible) continuous LP, then its objective
+        optimised over the plans that reach it (repair.py, DESIGN.md section 2k)."""
+        return _repair(self, model, weights, objective=objective, gap=gap, absolute_gap=absolute_gap,
+                       precision=precision, validate=validate)
+
     def _instance(self, model: Any, precision: Optional[float]) -> Model:
         if isinstance(model, dict):
             options = model.get("options") or {}
@@ -127,3 +135,9 @@ def Frontier(model: dict, precision: Optional[float] = None, validate: bool = Fa
 def Lexicographic(model: dict, gap=0.0, absolute_gap=0.0, precision: Optional[float] = None,
                   validate: bool = False) -> dict:
     return solver.Lexicographic(model, gap, absolute_gap, precision, validate)
+
+
+def Repair(model: dict, weights=None, *, objective: bool = True, gap=0.0, absolute_gap=0.0,
+           precision: Optional[float] = None, validate: bool = False) -> dict:
+    return solver.Repair(model, weights, objective=objective, gap=gap, absolute_gap=absolute_gap,
+                         precision=precision, validate=validate)

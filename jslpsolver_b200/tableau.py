@@ -786,6 +786,28 @@ class GpuTableau:
         f._refresh_dims()
         return f, kept
 
+    def elastic(self, rows, weights):
+        """jslp_elastic_create: (elastic, crashed).  `elastic` is a GpuTableau of this tableau, as upload() left it,
+        with one violation column per row of `rows` (increasing, in 1..height-1) weighted by `weights`, the rows that
+        start infeasible crashed onto their column, and row 0 the weighted total violation (DESIGN.md section 2k).  Its
+        labels are this tableau's plus len(rows) new ones from max(nVars, lastElementIndex); `crashed` counts the
+        crashed rows.  The copy stays on the device; this tableau is only read.  close() it when done."""
+        r = np.ascontiguousarray(rows, dtype=np.int32)
+        w = np.ascontiguousarray(weights, dtype=np.float64)
+        if len(r) != len(w):
+            raise ValueError(f"elastic: {len(r)} rows but {len(w)} weights")
+        h, n = C.c_void_p(), C.c_int32()
+        _lib.check(self.context.lib.jslp_elastic_create(self._h(), r.ctypes.data if len(r) else None,
+                                                        w.ctypes.data if len(w) else None, len(r), C.byref(h),
+                                                        C.byref(n)))
+        e = GpuTableau(self.precision, context=self.context)
+        e.handle = h
+        e.model, e.variablesPerIndex = self.model, self.variablesPerIndex
+        e.nOpt, e.nInts = 0, getattr(self, "nInts", 0)
+        e.engine, e.options = self.engine, dict(self.options)
+        e._refresh_dims()
+        return e, n.value
+
     def crash(self, enter, leave):
         """jslp_crash: pivot the labels `enter` into the basis in order, each on the row with the largest |entry| among
         the rows whose basic label has leave[label] != 0 (DESIGN.md section 2f).  Returns the records (n x 4: label,
