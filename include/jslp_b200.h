@@ -330,6 +330,35 @@ int jslp_lex_next(jslp_tab *tab, const double *cost_by_label, double allowance, 
 int jslp_elastic_create(jslp_tab *tab, const int32_t *rows, const double *weights, int n_rows, jslp_tab **elastic,
                         int32_t *n_crashed);
 
+/* The recession cone of an LP, DESIGN.md section 2l: a sibling tab in the same context.  With M the tab (H x W, as
+ * jslp_tab_upload left it) and l* = max(n_index, lastElementIndex), the new tab K is (H+1) x W: rows 0..H-1 are M's
+ * rows bit for bit except column 0, which is +0 in every one of them; row H is 1.0 at column 0 and at every column
+ * 1..W-1 (the normalisation sum_j d_j <= 1), +0 padding.  Its row labels are M's followed by l*, its column labels
+ * M's; precision, unrestricted / integer tables (l* restricted, not integer), element indices and options are the
+ * parent's, with lastElementIndex = l* + 1.  K's slack basis is primal feasible, and its optimum is non-zero exactly
+ * when M has an improving direction d >= 0 (every row's activity rate at most 0 towards its bound).
+ *   cone   the new tab (free it with jslp_tab_destroy)
+ * The copy runs device to device; the parent is only read.  No optional objectives (JSLP_E_UNSUPPORTED). */
+int jslp_cone_create(jslp_tab *tab, jslp_tab **cone);
+
+/* simplex() (cycle check on) of column subsets of the saved snapshot, DESIGN.md section 2l: set i writes +0 over every
+ * column c in 1..W-1 with keep_cols[i * W + c] == 0, in every row, row 0 included, and solves.  Sets whose tableau
+ * fits shared memory run one CTA each in one launch; the others, and any set whose pivot log shows a cycle or that hits
+ * the in-kernel pivot or log cap, run one after another on the single-tableau path (restore, zero, simplex).
+ *   keep_cols      n_sets x W bytes, nonzero = keep (column 0 is always kept)
+ *   status         per set: 0 optimal, 1 unbounded, 2 cycled (stopped before the pivot that completes the repeat),
+ *                  3 infeasible (only when the snapshot does not start primal feasible)
+ *   eval_raw       per set: the final M[0,0];  pivots: per set, phase-1 plus phase-2 pivots
+ *   rhs, vrow      n_sets x H: the final column 0 and row labels of each set
+ * Needs a snapshot (jslp_save); on return the tableau equals it, and the scalar Tableau state and executed-pivot log
+ * are as they were.  No optional objectives (JSLP_E_UNSUPPORTED). */
+int jslp_column_batch(jslp_tab *tab, const uint8_t *keep_cols, int n_sets, int32_t *status, double *eval_raw,
+                      int32_t *pivots, double *rhs, int32_t *vrow);
+
+/* Column `col` (0..W-1) of the current tableau, H doubles, into out: one strided device-to-host copy, so a single
+ * column of a large tableau is read without downloading the whole of it. */
+int jslp_column(jslp_tab *tab, int col, double *out);
+
 /* Multi-GPU communicator of the branch-and-cut frontier (one process per GPU).  NCCL is loaded at run time;
  * without libnccl these calls fail with JSLP_E_UNSUPPORTED and single-GPU use is unaffected.  Rank 0 obtains a
  * 128-byte unique id and hands it to the other ranks through whatever bootstrap the host has (the N-API host:

@@ -111,6 +111,9 @@ SYMBOLS = [
     ("jslp_bound_create", C.c_int, [P, C.c_double, C.POINTER(P)]),
     ("jslp_lex_next", C.c_int, [P, P, C.c_double, C.POINTER(P), C.POINTER(C.c_int32), P]),
     ("jslp_elastic_create", C.c_int, [P, P, P, C.c_int, C.POINTER(P), C.POINTER(C.c_int32)]),
+    ("jslp_cone_create", C.c_int, [P, C.POINTER(P)]),
+    ("jslp_column_batch", C.c_int, [P, P, C.c_int, P, P, P, P, P]),
+    ("jslp_column", C.c_int, [P, C.c_int, P]),
     ("jslp_branch_and_cut", C.c_int, [P, C.POINTER(BnbOpts), C.POINTER(BnbStatus), P, C.c_int]),
     ("jslp_bnb_node_log", C.c_int, [P, P, C.c_int64, C.POINTER(C.c_int64)]),
     ("jslp_bnb_solution", C.c_int, [P, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_int32), P, P, C.c_int]),

@@ -1379,3 +1379,4 @@ extern "C" int jslp_pivot_log(jslp_tab *t, int32_t *entries, int cap, int *n) {
 #include "jslp_bound.cuh"
 #include "jslp_lex.cuh"
 #include "jslp_elastic.cuh"
+#include "jslp_cone.cuh"

@@ -44,6 +44,7 @@ enum NodeMode : int {
     NODE_BRANCH = 0,    // branch-and-cut nodes and engine 4: every root row, then the node's cuts
     NODE_SUBSET = 1,    // one row subset of the root per CTA (jslp_feasibility_batch)
     NODE_SCENARIO = 2,  // one list of right-hand-side / cost edits of the root per CTA (jslp_scenario_batch)
+    NODE_COLUMNS = 3,   // one column subset of the root per CTA, the others zeroed (jslp_column_batch)
 };
 
 // One resolved scenario edit (DESIGN.md 2e): where updateRightHandSide / updateCost (dynamic-modification.ts:78-160)
@@ -71,12 +72,15 @@ struct NodeBatchDev {
     int H0, root_stride, first_index, Hcap, Ws, log_cap, max_pivots;
     // row-subset launches (NODE_SUBSET, jslp_feasibility_batch): node n keeps the root rows whose bits are set
     // in keep[n * keep_words ...] (device memory; row 0 is always kept), and with phase1_only the CTA stops with
-    // ST_P1_DONE where phase 1 finds no leaving row.  Not read by the other modes.
+    // ST_P1_DONE where phase 1 finds no leaving row.  Column-subset launches (NODE_COLUMNS, jslp_column_batch) read
+    // the same bits as columns: node n writes +0 over every column whose bit is clear, in every row.  Not read by
+    // the other modes.
     const uint32_t *keep;
     int keep_words, phase1_only;
     // scenario launches (NODE_SCENARIO, jslp_scenario_batch): node n applies edits[cut_off[n] .. cut_off[n+1]) (device
     // memory; every right-hand-side edit before every cost edit) to the restored root, solves, and writes its final
-    // column 0 and row labels to out_rhs / out_vrow + n * H0.  Not read by the other modes.
+    // column 0 and row labels to out_rhs / out_vrow + n * H0 (NODE_COLUMNS writes them too).  Not read by the other
+    // modes.
     const EditDev *edits;
     double *out_rhs;
     int *out_vrow;
@@ -142,11 +146,12 @@ struct NodePart {    // per-warp partial results of a scan
 // MODE = NODE_BRANCH: branch-and-cut nodes and engine 4 (every root row, then the node's cuts).  NODE_SUBSET: one row
 // subset of the root per CTA (NodeBatchDev.keep), compacted in row order; row labels stay the root's, so the
 // unrestricted lookup and the pivot log read as on the whole tableau.  NODE_SCENARIO: every root row, then the CTA's
-// edit list applied to column 0 and row 0 (DESIGN.md 2e) in place of cut rows.  A template parameter, so that the node
-// path carries none of the subset or scenario code.
+// edit list applied to column 0 and row 0 (DESIGN.md 2e) in place of cut rows.  NODE_COLUMNS: every root row, with the
+// columns cleared in the CTA's mask set to +0 in every row, row 0 included (DESIGN.md 2l).  A template parameter, so
+// that the node path carries none of the subset, scenario or column code.
 template <int MODE>
 __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, const __grid_constant__ NodeBatchDev nb) {
-    constexpr bool SUBSET = MODE == NODE_SUBSET, SCENARIO = MODE == NODE_SCENARIO;
+    constexpr bool SUBSET = MODE == NODE_SUBSET, SCENARIO = MODE == NODE_SCENARIO, COLUMNS = MODE == NODE_COLUMNS;
     extern __shared__ __align__(16) unsigned char smraw[];
     __shared__ TabDev T;
     __shared__ SelSmem sel;
@@ -216,12 +221,12 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
     const int W = T.W;
     const double prec = T.prec;
     int *vcol = T.vcol;
-    for (int h = tid; !SCENARIO && h < nc; h += NT) cutS[h] = nb.cuts[c0 + h];
+    for (int h = tid; !SCENARIO && !COLUMNS && h < nc; h += NT) cutS[h] = nb.cuts[c0 + h];
     for (int r = tid; r < H0k; r += NT) vrow[r] = __ldg(nb.root_vrow + (SUBSET ? slot[r] : r));
     for (int c = tid; c < W; c += NT) vcol[c] = __ldg(nb.root_vcol + c);
     if (!SUBSET)
         for (int r = tid; r < nb.Hcap; r += NT) slot[r] = r;
-    const int Hn = SCENARIO ? H0k : H0k + nc;
+    const int Hn = (SCENARIO || COLUMNS) ? H0k : H0k + nc;
     if (tid == 0) tl0 = globaltimer_ns() - t_start;
     mbar_wait(&s_bar, 0);
     __syncthreads();
@@ -254,9 +259,19 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
             Ms[c] = x;
         }
     }
+    if constexpr (COLUMNS) {
+        // the cleared columns of this CTA's mask are +0 in every row: a zero column prices at 0, so it never
+        // enters, and a pivot leaves it zero
+        const uint32_t *kw = nb.keep + (size_t)node * nb.keep_words;
+        for (int r = warp; r < Hn; r += NW) {
+            double *row = Ms + (size_t)r * Ws;
+            for (int c = 1 + lane; c < W; c += 32)
+                if (!((kw[c >> 5] >> (c & 31)) & 1u)) row[c] = 0.0;
+        }
+    }
     // addCutConstraints(): every cut row is expressed in the ROOT basis, so the rows are independent:
-    // one warp per cut, no CTA barrier inside (a scenario's nc counts edits)
-    for (int h = warp; !SCENARIO && h < nc; h += NW) {
+    // one warp per cut, no CTA barrier inside (a scenario's nc counts edits; a column launch has none)
+    for (int h = warp; !SCENARIO && !COLUMNS && h < nc; h += NW) {
         const CutDev cut = cutS[h];
         int s_row, s_col;
         cut_lookup(vrow, H0k, vcol, W, cut.var_index, lane, 32, s_row, s_col);
@@ -484,7 +499,7 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
     // isIntegral / most fractional variable over the final RHS column
     for (int r = tid; r < Hn; r += NT) rhs[r] = Ms[(size_t)slot[r] * Ws];
     __syncthreads();
-    if constexpr (SCENARIO)
+    if constexpr (SCENARIO || COLUMNS)
         for (int r = tid; r < Hn; r += NT) {
             nb.out_rhs[(size_t)node * H0 + r] = rhs[r];
             nb.out_vrow[(size_t)node * H0 + r] = vrow[r];

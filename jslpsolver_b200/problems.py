@@ -235,6 +235,49 @@ def infeasible_packing_model(n_vars: int, n_cons: int, n_demand: int, seed: int 
     return dict(lp_model(A, b, c, lower), name=f"InfeasiblePacking_{n_vars}x{n_cons}_{n_demand}_seed{seed}")
 
 
+def planted_unbounded_model(n_vars: int, n_cons: int, n_solo: int, n_pairs: int, seed: int = 12345) -> dict:
+    """max c.x over a dense packing LP with planted leaks, unbounded by construction.  n_vars and n_cons count every
+    variable and row.  The packing part has n_vars - n_solo - 2 n_pairs variables `x{j}` and n_cons - 2 n_pairs rows
+    a_i.x <= b_i with a_ij ~ U{1..20}, b_i ~ U{100..500}: every entry is positive, so it is bounded on its own.  A solo
+    leak `solo{k}` has no entry in any row.  A pair leak is `pairU{k}` and `pairV{k}` with the rows `u - v <= b1` and
+    `v - u <= b2` (b ~ U{1..10}): either variable alone is blocked by the other's cap, and u + v runs away.  Every cost
+    is U{1..50}.  The leak columns sit at seeded positions among the packing columns, u before v.  The irreducible set
+    the one-at-a-time deletion filter over the columns returns is every solo leak plus the v of each pair: a cap on v
+    alone bounds the pair, so the filter drops u first."""
+    rng = np.random.default_rng(seed)
+    n_pack, r_pack = n_vars - n_solo - 2 * n_pairs, n_cons - 2 * n_pairs
+    if n_pack < 0 or r_pack < 0 or (n_pack > 0 and r_pack == 0):
+        raise ValueError("planted_unbounded_model: more leaks than variables or rows, or no packing row")
+    kinds = ["x"] * n_pack + ["solo"] * n_solo + ["pair"] * n_pairs
+    order = rng.permutation(len(kinds))
+    A = rng.integers(1, 21, size=(r_pack, n_pack)).astype(np.float64)
+    b = rng.integers(100, 501, size=r_pack).astype(np.float64)
+    constraints = {f"resource{i}": {"max": float(b[i])} for i in range(r_pack)}
+    variables = {}
+    j = k_solo = k_pair = 0
+    for pos in order:
+        kind = kinds[pos]
+        if kind == "x":
+            v = {"profit": float(rng.integers(1, 51))}
+            for i in range(r_pack):
+                v[f"resource{i}"] = float(A[i, j])
+            variables[f"x{j}"] = v
+            j += 1
+        elif kind == "solo":
+            variables[f"solo{k_solo}"] = {"profit": float(rng.integers(1, 51))}
+            k_solo += 1
+        else:
+            k = k_pair
+            b1, b2 = rng.integers(1, 11, size=2)
+            constraints[f"pairA{k}"] = {"max": float(b1)}
+            constraints[f"pairB{k}"] = {"max": float(b2)}
+            variables[f"pairU{k}"] = {"profit": float(rng.integers(1, 51)), f"pairA{k}": 1.0, f"pairB{k}": -1.0}
+            variables[f"pairV{k}"] = {"profit": float(rng.integers(1, 51)), f"pairA{k}": -1.0, f"pairB{k}": 1.0}
+            k_pair += 1
+    return {"name": f"PlantedUnbounded_{n_vars}x{n_cons}_{n_solo}_{n_pairs}_seed{seed}", "optimize": "profit",
+            "opType": "max", "constraints": constraints, "variables": variables}
+
+
 def knapsack_mip_model(n_items: int, n_cons: int, seed: int = 12345, tolerance: float = 0.0) -> dict:
     """Multi-dimensional 0/1 knapsack (SURVEY.md 8d config 5): a_ij ~ U{1..50} dense,
     b_i = floor(0.5 * sum_j a_ij), c_j ~ U{1..50}; every binary adds an `x <= 1` row

@@ -108,6 +108,15 @@ class Solution:  # solution.ts:16-61
         from .iis import compute
         return compute(self)
 
+    def unbounded(self, width=None) -> dict:
+        """Why this continuous LP is unbounded (DESIGN.md section 2l): the improving ray where the simplex stopped,
+        {"ray", "rate", "point", "constraints", "blocking"}, whether a recession-cone LP confirms an improving direction
+        ("confirmed"), an irreducible set of variables whose caps make the LP bounded ("bound": {"variables",
+        "irreducible"}, None when undecided) and the cone LPs solved ("lps").  The tableau and the model are left
+        unchanged; raises ValueError where it is not defined.  `width` tunes the schedule only."""
+        from .unbounded import compute
+        return compute(self, width=width)
+
     def parametric(self, constraint=None, variable=None, side=None, to=None) -> dict:
         """The optimal result of this continuous LP as one right-hand side (constraint=name, side= for a constraint
         with a min and a max bound) or one cost (variable=id) moves from its current value to `to`: linear pieces
@@ -807,6 +816,45 @@ class GpuTableau:
         e.engine, e.options = self.engine, dict(self.options)
         e._refresh_dims()
         return e, n.value
+
+    def cone(self) -> "GpuTableau":
+        """jslp_cone_create: a GpuTableau of the recession cone of this tableau, as upload() left it -- column 0 set to
+        +0, and one last row sum_j d_j <= 1 over the columns with one new row label, max(nVars, lastElementIndex) --
+        with this tableau's column labels, options and model (DESIGN.md section 2l).  The copy stays on the device;
+        this tableau is only read.  close() it when done."""
+        h = C.c_void_p()
+        _lib.check(self.context.lib.jslp_cone_create(self._h(), C.byref(h)))
+        k = GpuTableau(self.precision, context=self.context)
+        k.handle = h
+        k.model, k.variablesPerIndex = self.model, self.variablesPerIndex
+        k.nOpt, k.nInts = 0, getattr(self, "nInts", 0)
+        k.engine, k.options = self.engine, dict(self.options)
+        k._refresh_dims()
+        return k
+
+    def column_batch(self, keep_cols) -> dict:
+        """jslp_column_batch: simplex() (cycle check on) of the saved snapshot with the columns not kept in keep[s]
+        (n_sets x width, nonzero = keep; column 0 is always kept) set to +0 in every row (DESIGN.md section 2l).
+        Returns the per-set status (0 optimal, 1 unbounded, 2 cycled, 3 infeasible), raw M[0,0], pivots, and the final
+        right-hand-side column and row labels (n x height).  Leaves the tableau equal to its snapshot."""
+        keep = np.ascontiguousarray(keep_cols, dtype=np.uint8)
+        n, H = keep.shape[0], self.height
+        if n and keep.shape[1] != self.width:
+            raise ValueError(f"column_batch: masks have {keep.shape[1]} columns, the tableau {self.width}")
+        status, pivots = np.empty(n, dtype=np.int32), np.empty(n, dtype=np.int32)
+        eval_raw = np.empty(n, dtype=np.float64)
+        rhs, vrow = np.empty((n, H), dtype=np.float64), np.empty((n, H), dtype=np.int32)
+        _lib.check(self.context.lib.jslp_column_batch(self._h(), keep.ctypes.data, n, status.ctypes.data,
+                                                      eval_raw.ctypes.data, pivots.ctypes.data, rhs.ctypes.data,
+                                                      vrow.ctypes.data))
+        self._refresh_dims()
+        return {"status": status, "eval_raw": eval_raw, "pivots": pivots, "rhs": rhs, "vrow": vrow}
+
+    def column(self, col: int) -> np.ndarray:
+        """jslp_column: column `col` of the current tableau (height doubles), without downloading the rest."""
+        out = np.empty(self.height, dtype=np.float64)
+        _lib.check(self.context.lib.jslp_column(self._h(), int(col), out.ctypes.data))
+        return out
 
     def crash(self, enter, leave):
         """jslp_crash: pivot the labels `enter` into the basis in order, each on the row with the largest |entry| among
