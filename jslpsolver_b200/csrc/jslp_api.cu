@@ -17,6 +17,7 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <unordered_map>
 #include <vector>
@@ -168,10 +169,10 @@ struct jslp_tab {
     long long node_kernel_ns = 0;  // sum over rounds of the slowest node CTA (reporting)
     unsigned long long *d_sens = nullptr;  // jslp_sensitivity's key buffers: 2 x sens_cap
     size_t sens_cap = 0;
-    void *d_iis = nullptr;  // jslp_feasibility_batch: packed keep masks / the gathered row list
-    size_t iis_bytes = 0;
-    void *d_scen = nullptr;  // jslp_scenario_batch: offsets, resolved edits and per-scenario outputs of one chunk
-    size_t scen_bytes = 0;
+    // jslp_feasibility_batch / jslp_scenario_batch / jslp_column_batch (batch_scratch): keep masks, the gathered row
+    // list, or one chunk's offsets, resolved edits and per-set outputs
+    void *d_scratch = nullptr;
+    size_t scratch_bytes = 0;
     void *d_param = nullptr, *d_plog = nullptr;  // jslp_parametric: path state and its breakpoint log
     int param_cap = 0;
     cudaGraphExec_t param_graph = nullptr;
@@ -346,7 +347,7 @@ extern "C" void jslp_tab_destroy(jslp_tab *t) {
     cudaFree(t->d_T); cudaFree(t->d_rec); cudaFree(t->d_mip); cudaFree(t->d_cuts);
     cudaFreeHost(t->h_rec); cudaFreeHost(t->h_log); cudaFreeHost(t->h_mip); cudaFreeHost(t->h_cuts);
     cudaFree(t->d_count); cudaFreeHost(t->h_count);
-    cudaFree(t->d_sens); cudaFree(t->d_iis); cudaFree(t->d_scen);
+    cudaFree(t->d_sens); cudaFree(t->d_scratch);
     cudaFree(t->d_param); cudaFree(t->d_plog); cudaFree(t->d_front);
     if (t->param_graph) cudaGraphExecDestroy(t->param_graph);
     cudaFree(t->d_crash); cudaFree(t->d_crash_buf);

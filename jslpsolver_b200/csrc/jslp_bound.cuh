@@ -39,6 +39,28 @@ __global__ void __launch_bounds__(BOUND_THREADS) k_bound_rows(const TabDev *Tp, 
 
 }  // namespace jslp
 
+// Rows [r0, H) of t's current buffer into the same rows of its sibling c, and t's row and column labels.  The
+// ping-pong step swaps TabDev.M / M2 on the device, so the source is the device's view of "current".
+static int sibling_copy_rows(const jslp_tab *t, jslp_tab *c, int r0) {
+    cudaStream_t s = t->ctx->stream;
+    const int W = t->W, H = t->H;
+    TabDev cur;
+    CK(cudaMemcpyAsync(&cur, t->d_T, sizeof(TabDev), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    if (H > r0) {
+        if (c->stride == t->stride)
+            CK(cudaMemcpyAsync(c->hd.M + (size_t)r0 * c->stride, cur.M + (size_t)r0 * t->stride,
+                               sizeof(double) * (size_t)(H - r0) * t->stride, cudaMemcpyDeviceToDevice, s));
+        else  // a parent that removeVariable left wider than ceil16(W): its logical width, row by row
+            CK(cudaMemcpy2DAsync(c->hd.M + (size_t)r0 * c->stride, sizeof(double) * c->stride,
+                                 cur.M + (size_t)r0 * t->stride, sizeof(double) * t->stride, sizeof(double) * W, H - r0,
+                                 cudaMemcpyDeviceToDevice, s));
+    }
+    CK(cudaMemcpyAsync(c->hd.vrow, t->hd.vrow, sizeof(int) * (size_t)H, cudaMemcpyDeviceToDevice, s));
+    CK(cudaMemcpyAsync(c->hd.vcol, t->hd.vcol, sizeof(int) * (size_t)W, cudaMemcpyDeviceToDevice, s));
+    return JSLP_OK;
+}
+
 // The bound tableau of t into *out.  With d_cost (a device array of C by label) row 0 is the next objective priced
 // against t at every column (k_price_objective, section 2j) instead of +0.
 static int bound_build(jslp_tab *t, double allowance, const double *d_cost, jslp_tab **out) {
@@ -46,50 +68,24 @@ static int bound_build(jslp_tab *t, double allowance, const double *d_cost, jslp
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = ctx->stream;
     const int W = t->W, H = t->H;
-    const int label = std::max(t->n_index, t->lastElementIndex);
-    // the ping-pong step swaps TabDev.M / M2 on the device: copy from the device's view of "current"
-    TabDev cur;
-    CK(cudaMemcpyAsync(&cur, t->d_T, sizeof(TabDev), cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    jslp_tab *b = nullptr;
-    // CK returns: release what this call owns on the way out
-    auto body = [&]() -> int {
-        int rc = jslp_tab_create(ctx, W, H + 1, std::max(t->rowcap, H + 1), t->precision, &b);
-        if (rc) return rc;
-        b->nVars = t->nVars + 1; b->lastElementIndex = label + 1;  // cut rows would take labels after l*
-        rc = inherit_tables_and_options(t, b, label + 1);
-        if (rc) return rc;
-        rc = push_desc(b);
-        if (rc) return rc;
-        if (H > 1) {
-            if (b->stride == t->stride)
-                CK(cudaMemcpyAsync(b->hd.M + b->stride, cur.M + t->stride, sizeof(double) * (size_t)(H - 1) * t->stride,
-                                   cudaMemcpyDeviceToDevice, s));
-            else  // a parent that removeVariable left wider than ceil16(W): its logical width, row by row
-                CK(cudaMemcpy2DAsync(b->hd.M + b->stride, sizeof(double) * b->stride, cur.M + t->stride,
-                                     sizeof(double) * t->stride, sizeof(double) * W, H - 1, cudaMemcpyDeviceToDevice, s));
-        }
-        CK(cudaMemcpyAsync(b->hd.vrow, t->hd.vrow, sizeof(int) * (size_t)H, cudaMemcpyDeviceToDevice, s));
-        CK(cudaMemcpyAsync(b->hd.vcol, t->hd.vcol, sizeof(int) * (size_t)W, cudaMemcpyDeviceToDevice, s));
-        k_bound_rows<<<(b->stride + BOUND_THREADS - 1) / BOUND_THREADS, BOUND_THREADS, 0, s>>>(t->d_T, allowance, b->hd.M,
-                                                                                              b->stride, b->hd.vrow, label);
+    const int label = first_free_label(t);
+    TabOwner b;
+    int rc = sibling_create(t, W, H + 1, 1, b);
+    if (rc) return rc;
+    rc = sibling_copy_rows(t, b.get(), 1);
+    if (rc) return rc;
+    k_bound_rows<<<(b->stride + BOUND_THREADS - 1) / BOUND_THREADS, BOUND_THREADS, 0, s>>>(t->d_T, allowance, b->hd.M,
+                                                                                          b->stride, b->hd.vrow, label);
+    ctx->launches += 1;
+    CK(cudaGetLastError());
+    if (d_cost) {  // over the +0 k_bound_rows wrote at columns 0..W-1; the padding stays +0
+        k_price_objective<<<(W + FR_COLS - 1) / FR_COLS, FR_COLS, 0, s>>>(t->d_T, d_cost, nullptr, W, b->hd.M,
+                                                                          nullptr);
         ctx->launches += 1;
         CK(cudaGetLastError());
-        if (d_cost) {  // over the +0 k_bound_rows wrote at columns 0..W-1; the padding stays +0
-            k_price_objective<<<(W + FR_COLS - 1) / FR_COLS, FR_COLS, 0, s>>>(t->d_T, d_cost, nullptr, W, b->hd.M,
-                                                                              nullptr);
-            ctx->launches += 1;
-            CK(cudaGetLastError());
-        }
-        CK(cudaStreamSynchronize(s));
-        return JSLP_OK;
-    };
-    const int rc = body();
-    if (rc) {
-        if (b) jslp_tab_destroy(b);
-        return rc;
     }
-    *out = b;
+    CK(cudaStreamSynchronize(s));
+    *out = b.release();
     return JSLP_OK;
 }
 

@@ -48,41 +48,19 @@ extern "C" int jslp_cone_create(jslp_tab *t, jslp_tab **out) {
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = ctx->stream;
     const int W = t->W, H = t->H;
-    const int label = std::max(t->n_index, t->lastElementIndex);
-    // the ping-pong step swaps TabDev.M / M2 on the device: copy from the device's view of "current"
-    TabDev cur;
-    CK(cudaMemcpyAsync(&cur, t->d_T, sizeof(TabDev), cudaMemcpyDeviceToHost, s));
+    const int label = first_free_label(t);
+    TabOwner k;
+    int rc = sibling_create(t, W, H + 1, 1, k);
+    if (rc) return rc;
+    rc = sibling_copy_rows(t, k.get(), 0);
+    if (rc) return rc;
+    const int n = std::max(H, k->stride);
+    k_cone_rows<<<(n + CONE_THREADS - 1) / CONE_THREADS, CONE_THREADS, 0, s>>>(k->hd.M, k->stride, W, H, k->hd.vrow,
+                                                                              label);
+    ctx->launches += 1;
+    CK(cudaGetLastError());
     CK(cudaStreamSynchronize(s));
-    jslp_tab *k = nullptr;
-    auto body = [&]() -> int {
-        int rc = jslp_tab_create(ctx, W, H + 1, std::max(t->rowcap, H + 1), t->precision, &k);
-        if (rc) return rc;
-        k->nVars = t->nVars + 1; k->lastElementIndex = label + 1;  // cut rows would take labels after l*
-        rc = inherit_tables_and_options(t, k, label + 1);
-        if (rc) return rc;
-        rc = push_desc(k);
-        if (rc) return rc;
-        if (k->stride == t->stride)
-            CK(cudaMemcpyAsync(k->hd.M, cur.M, sizeof(double) * (size_t)H * t->stride, cudaMemcpyDeviceToDevice, s));
-        else  // a parent that removeVariable left wider than ceil16(W): its logical width, row by row
-            CK(cudaMemcpy2DAsync(k->hd.M, sizeof(double) * k->stride, cur.M, sizeof(double) * t->stride,
-                                 sizeof(double) * W, H, cudaMemcpyDeviceToDevice, s));
-        CK(cudaMemcpyAsync(k->hd.vrow, t->hd.vrow, sizeof(int) * (size_t)H, cudaMemcpyDeviceToDevice, s));
-        CK(cudaMemcpyAsync(k->hd.vcol, t->hd.vcol, sizeof(int) * (size_t)W, cudaMemcpyDeviceToDevice, s));
-        const int n = std::max(H, k->stride);
-        k_cone_rows<<<(n + CONE_THREADS - 1) / CONE_THREADS, CONE_THREADS, 0, s>>>(k->hd.M, k->stride, W, H, k->hd.vrow,
-                                                                                  label);
-        ctx->launches += 1;
-        CK(cudaGetLastError());
-        CK(cudaStreamSynchronize(s));
-        return JSLP_OK;
-    };
-    const int rc = body();
-    if (rc) {
-        if (k) jslp_tab_destroy(k);
-        return rc;
-    }
-    *out = k;
+    *out = k.release();
     return JSLP_OK;
 }
 
@@ -94,10 +72,10 @@ static int column_hbm(jslp_tab *t, const uint32_t *bits, int words, int32_t *sta
     cudaStream_t s = t->ctx->stream;
     int rc = jslp_restore(t);
     if (rc) return rc;
-    rc = iis_scratch(t, sizeof(uint32_t) * (size_t)words);
+    rc = batch_scratch(t, sizeof(uint32_t) * (size_t)words);
     if (rc) return rc;
-    CK(cudaMemcpyAsync(t->d_iis, bits, sizeof(uint32_t) * (size_t)words, cudaMemcpyHostToDevice, s));
-    k_zero_columns<<<std::min(t->H, t->ctx->num_sms * 4), CONE_THREADS, 0, s>>>(t->d_T, (const uint32_t *)t->d_iis);
+    CK(cudaMemcpyAsync(t->d_scratch, bits, sizeof(uint32_t) * (size_t)words, cudaMemcpyHostToDevice, s));
+    k_zero_columns<<<std::min(t->H, t->ctx->num_sms * 4), CONE_THREADS, 0, s>>>(t->d_T, (const uint32_t *)t->d_scratch);
     t->ctx->launches += 1;
     CK(cudaGetLastError());
     jslp_lp_status st;
@@ -106,66 +84,41 @@ static int column_hbm(jslp_tab *t, const uint32_t *bits, int words, int32_t *sta
     *status = st.cycled ? COL_CYCLED : !st.feasible ? COL_INFEASIBLE : !st.bounded ? COL_UNBOUNDED : COL_OPTIMAL;
     *eval_raw = st.evaluation_raw;
     *pivots = st.phase1_pivots + st.phase2_pivots;
-    CK(cudaMemcpy2DAsync(rhs, sizeof(double), t->hd.M, sizeof(double) * t->stride, sizeof(double), t->H,
-                         cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(vrow, t->hd.vrow, sizeof(int) * (size_t)t->H, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    return JSLP_OK;
+    return read_column(t, 0, rhs, vrow);
 }
 
 // Sets [s0, s0 + n) in one k_node_batch<NODE_COLUMNS> launch.  Those whose log shows a cycle (per-phase histories) or
 // that hit the pivot or log cap go to redo: the HBM path stops a cycle before the pivot that completes the repeat.
 static int column_resident(jslp_tab *t, const uint32_t *bits, int words, int s0, int n, int32_t *status,
                            double *eval_raw, int32_t *pivots, double *rhs, int32_t *vrow, std::vector<int> &redo) {
-    jslp_ctx *ctx = t->ctx;
-    cudaStream_t s = ctx->stream;
     ResidentBufs &rb = t->rbufs;
     const int H0 = t->saved.H;
-    int Ws = 0;
-    const size_t smem = node_smem_bytes(H0, t->W, &Ws);
-    const int log_cap = t->node_log_cap;
-    int rc = rb.ensure(n, 0, log_cap);
+    NodeBatchDev nb;
+    size_t smem = 0;
+    int rc = batch_fill(t, t->saved.M, t->saved.vrow, t->saved.vcol, H0, t->saved.lastElementIndex, n, nb, &smem);
     if (rc) return rc;
     for (int i = 0; i <= n; i++) rb.h_off[i] = 0;  // no cut rows
+    nb.cuts = rb.dv_cuts; nb.cut_off = rb.dv_off;
     // one device block per chunk: masks, final columns, final labels
     const size_t b_rhs = (sizeof(uint32_t) * (size_t)n * words + 15) & ~(size_t)15;
     const size_t b_vrow = b_rhs + sizeof(double) * (size_t)n * H0;
-    rc = iis_scratch(t, b_vrow + sizeof(int) * (size_t)n * H0);
+    rc = batch_scratch(t, b_vrow + sizeof(int) * (size_t)n * H0);
     if (rc) return rc;
-    char *base = (char *)t->d_iis;
-    CK(cudaMemcpyAsync(base, bits + (size_t)s0 * words, sizeof(uint32_t) * (size_t)n * words, cudaMemcpyHostToDevice, s));
-    NodeBatchDev nb;
-    memset(&nb, 0, sizeof(nb));
-    nb.rootM = t->saved.M; nb.root_vrow = t->saved.vrow; nb.root_vcol = t->saved.vcol;
-    nb.cuts = rb.dv_cuts; nb.cut_off = rb.dv_off; nb.out = rb.dv_out; nb.logs = rb.d_logs;
-    nb.H0 = H0; nb.root_stride = t->stride; nb.first_index = t->saved.lastElementIndex;
-    nb.Hcap = H0; nb.Ws = Ws; nb.log_cap = log_cap; nb.max_pivots = 100000;
+    char *base = (char *)t->d_scratch;
+    CK(cudaMemcpyAsync(base, bits + (size_t)s0 * words, sizeof(uint32_t) * (size_t)n * words, cudaMemcpyHostToDevice,
+                       t->ctx->stream));
     nb.keep = (const uint32_t *)base; nb.keep_words = words;
     nb.out_rhs = (double *)(base + b_rhs); nb.out_vrow = (int *)(base + b_vrow);
     if (n <= NODE_INLINE_OFF) nb.n_inline = n;  // cut_off_inline: all zero
-    CK(cudaFuncSetAttribute(k_node_batch<NODE_COLUMNS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k_node_batch<NODE_COLUMNS><<<n, NODE_THREADS, smem, s>>>(t->d_T, nb);
-    ctx->launches += 1;
-    CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(rhs + (size_t)s0 * H0, nb.out_rhs, sizeof(double) * (size_t)n * H0, cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(vrow + (size_t)s0 * H0, nb.out_vrow, sizeof(int) * (size_t)n * H0, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
+    rc = batch_launch<NODE_COLUMNS>(t, nb, n, smem, rhs + (size_t)s0 * H0, vrow + (size_t)s0 * H0);
+    if (rc) return rc;
     bool need_full = false;
     for (int i = 0; i < n; i++) need_full |= !rb.h_out[i].r.overflow && rb.h_out[i].r.log_n > NODE_LOG_HEAD;
-    if (need_full) {
-        CK(cudaMemcpyAsync(rb.h_logs, rb.d_logs, sizeof(int4) * (size_t)n * log_cap, cudaMemcpyDeviceToHost, s));
-        CK(cudaStreamSynchronize(s));
-    }
+    rc = batch_fetch_logs(t, n, need_full);
+    if (rc) return rc;
     for (int i = 0; i < n; i++) {
         const NodeResult &r = rb.h_out[i].r;
-        bool again = r.overflow != 0;
-        if (!again) {
-            CycleHist h[2];  // (leaving, entering) per phase (simplex.ts:27,102)
-            int cs, cl;
-            const int4 *lg = r.log_n > NODE_LOG_HEAD ? rb.h_logs + (size_t)i * log_cap : rb.h_out[i].log_head;
-            for (int k = 0; k < r.log_n && k < log_cap && !again; k++)
-                again = h[((lg[k].x >> 30) & 1) ? 1 : 0].push_and_check(((long long)lg[k].z << 32) | (unsigned int)lg[k].w, &cs, &cl);
-        }
+        const bool again = r.overflow || first_cycle(batch_log(t, i), std::min(r.log_n, t->node_log_cap)) >= 0;
         if (again) { redo.push_back(s0 + i); continue; }
         status[s0 + i] = r.status == ST_OPTIMAL ? COL_OPTIMAL : r.status == ST_UNBOUNDED ? COL_UNBOUNDED : COL_INFEASIBLE;
         eval_raw[s0 + i] = r.eval_raw;
@@ -190,15 +143,11 @@ extern "C" int jslp_column_batch(jslp_tab *t, const uint8_t *keep_cols, int n_se
     for (int i = 0; i < n_sets; i++)
         for (int c = 0; c < W; c++)
             if (c == 0 || keep_cols[(size_t)i * W + c]) bits[(size_t)i * words + (c >> 5)] |= 1u << (c & 31);
-    // the scalar Tableau state and the executed-pivot log describe the tableau, not these tests
-    const int feasible = t->feasible, bounded = t->bounded, iters = t->simplexIters, unb = t->unboundedVar;
-    const double evaluation = t->evaluation, best = t->bestPossibleEval;
-    const size_t log_size = t->host_log.size();
+    const CallerState caller(t);
     std::vector<int> redo;
     int rc = JSLP_OK;
-    if (t->engine != 1 && t->engine != 2 && resident_fits(t, H0)) {
-        // chunks keep the per-set outputs on the device bounded (about 32 MB)
-        const int chunk = (int)std::max<size_t>(1, std::min<size_t>(4096, ((size_t)32 << 20) / ((size_t)12 * H0)));
+    if (batch_resident(t, H0)) {
+        const int chunk = batch_chunk(H0);
         for (int s0 = 0; s0 < n_sets && rc == JSLP_OK; s0 += chunk)
             rc = column_resident(t, bits.data(), words, s0, std::min(chunk, n_sets - s0), status, eval_raw, pivots, rhs,
                                  vrow, redo);
@@ -213,9 +162,7 @@ extern "C" int jslp_column_batch(jslp_tab *t, const uint8_t *keep_cols, int n_se
     const int rc2 = jslp_restore(t);
     if (rc == JSLP_OK) rc = rc2;
     CK(cudaStreamSynchronize(t->ctx->stream));
-    t->feasible = feasible; t->bounded = bounded; t->simplexIters = iters; t->unboundedVar = unb;
-    t->evaluation = evaluation; t->bestPossibleEval = best;
-    if (t->host_log.size() > log_size) t->host_log.resize(log_size);
+    caller.restore(t);
     return rc;
 }
 
@@ -223,10 +170,5 @@ extern "C" int jslp_column(jslp_tab *t, int col, double *out) {
     if (!t || !out) return fail(JSLP_E_INVALID, "NULL argument");
     if (col < 0 || col >= t->W) return fail(JSLP_E_INVALID, "column: index out of range");
     CK(cudaSetDevice(t->ctx->device));
-    cudaStream_t s = t->ctx->stream;
-    // the host mirror's M is the device's current buffer between calls (run_lp adopts it after every solve)
-    CK(cudaMemcpy2DAsync(out, sizeof(double), t->hd.M + col, sizeof(double) * t->stride, sizeof(double), t->H,
-                         cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    return JSLP_OK;
+    return read_column(t, col, out, nullptr);
 }

@@ -140,65 +140,53 @@ extern "C" int jslp_elastic_create(jslp_tab *t, const int32_t *rows, const doubl
             return fail(JSLP_E_INVALID, "elastic_create: row " + std::to_string(r) +
                                             " does not have its own slack basic (the tab must be as uploaded)");
     }
-    const int label = std::max(t->n_index, t->lastElementIndex);
+    const int label = first_free_label(t);
     const int tiles = (H - 1 + ELASTIC_TILE_ROWS - 1) / ELASTIC_TILE_ROWS;
-    jslp_tab *e = nullptr;
-    int rc = jslp_tab_create(ctx, W + k, H, std::max(t->rowcap, H), t->precision, &e);
+    TabOwner e;
+    int rc = sibling_create(t, W + k, H, k, e);  // cut rows would take labels after l*+k-1
     if (rc) return rc;
     const int estride = e->stride;
     // one scratch block: w[k] and part[tiles x estride] (doubles), then jof[H], rows[k], crashed[k], count (ints)
     const size_t n_dbl = (size_t)k + (size_t)std::max(tiles, 1) * estride;
     const size_t n_int = (size_t)H + 2 * (size_t)k + 1;
     void *d_buf = nullptr;
-    auto body = [&]() -> int {
-        e->nVars = t->nVars + k; e->lastElementIndex = label + k;  // cut rows would take labels after l*+k-1
-        int rc2 = inherit_tables_and_options(t, e, label + k);
-        if (rc2) return rc2;
-        rc2 = push_desc(e);
-        if (rc2) return rc2;
-        CK(cudaMalloc(&d_buf, sizeof(double) * n_dbl + sizeof(int) * n_int));
-        ElasticArgs a;
-        double *d_w = (double *)d_buf;
-        a.w = d_w;
-        a.part = d_w + k;
-        int *d_jof = (int *)(d_w + n_dbl);
-        a.jof = d_jof;
-        a.rows = d_jof + H;
-        a.crashed = d_jof + H + k;
-        a.count = d_jof + H + 2 * k;
-        a.E = e->hd.M; a.vrow = e->hd.vrow; a.vcol = e->hd.vcol;
-        a.k = k; a.estride = estride; a.label = label;
-        std::vector<int> ints(n_int, -1);
-        for (int j = 0; j < k; j++) {
-            ints[(size_t)rows[j]] = j;
-            ints[(size_t)H + j] = rows[j];
-        }
-        ints[n_int - 1] = 0;
-        CK(cudaMemcpyAsync(d_jof, ints.data(), sizeof(int) * n_int, cudaMemcpyHostToDevice, s));
-        if (k > 0) CK(cudaMemcpyAsync(d_w, weights, sizeof(double) * (size_t)k, cudaMemcpyHostToDevice, s));
-        if (tiles > 0) {
-            const dim3 grid((unsigned)(estride / ELASTIC_COLS + (estride % ELASTIC_COLS != 0)), (unsigned)tiles);
-            k_elastic_rows<<<grid, ELASTIC_COLS, 0, s>>>(t->d_T, a);
-            ctx->launches += 1;
-            CK(cudaGetLastError());
-        } else {  // no row below the cost row: only the labels of row 0 and the columns
-            CK(cudaMemcpyAsync(e->hd.vrow, t->hd.vrow, sizeof(int), cudaMemcpyDeviceToDevice, s));
-            CK(cudaMemcpyAsync(e->hd.vcol, t->hd.vcol, sizeof(int) * (size_t)W, cudaMemcpyDeviceToDevice, s));
-        }
-        k_elastic_cost<<<(estride + ELASTIC_COLS - 1) / ELASTIC_COLS, ELASTIC_COLS, 0, s>>>(W, tiles, a);
+    CK(cudaMalloc(&d_buf, sizeof(double) * n_dbl + sizeof(int) * n_int));
+    const std::unique_ptr<void, DevFree> buf(d_buf);
+    ElasticArgs a;
+    double *d_w = (double *)d_buf;
+    a.w = d_w;
+    a.part = d_w + k;
+    int *d_jof = (int *)(d_w + n_dbl);
+    a.jof = d_jof;
+    a.rows = d_jof + H;
+    a.crashed = d_jof + H + k;
+    a.count = d_jof + H + 2 * k;
+    a.E = e->hd.M; a.vrow = e->hd.vrow; a.vcol = e->hd.vcol;
+    a.k = k; a.estride = estride; a.label = label;
+    std::vector<int> ints(n_int, -1);
+    for (int j = 0; j < k; j++) {
+        ints[(size_t)rows[j]] = j;
+        ints[(size_t)H + j] = rows[j];
+    }
+    ints[n_int - 1] = 0;
+    CK(cudaMemcpyAsync(d_jof, ints.data(), sizeof(int) * n_int, cudaMemcpyHostToDevice, s));
+    if (k > 0) CK(cudaMemcpyAsync(d_w, weights, sizeof(double) * (size_t)k, cudaMemcpyHostToDevice, s));
+    if (tiles > 0) {
+        const dim3 grid((unsigned)(estride / ELASTIC_COLS + (estride % ELASTIC_COLS != 0)), (unsigned)tiles);
+        k_elastic_rows<<<grid, ELASTIC_COLS, 0, s>>>(t->d_T, a);
         ctx->launches += 1;
         CK(cudaGetLastError());
-        CK(cudaMemcpyAsync(n_crashed, a.count, sizeof(int), cudaMemcpyDeviceToHost, s));
-        CK(cudaStreamSynchronize(s));
-        return JSLP_OK;
-    };
-    rc = body();
-    cudaFree(d_buf);
-    if (rc) {
-        jslp_tab_destroy(e);
-        *n_crashed = 0;
-        return rc;
+    } else {  // no row below the cost row: only the labels of row 0 and the columns
+        CK(cudaMemcpyAsync(e->hd.vrow, t->hd.vrow, sizeof(int), cudaMemcpyDeviceToDevice, s));
+        CK(cudaMemcpyAsync(e->hd.vcol, t->hd.vcol, sizeof(int) * (size_t)W, cudaMemcpyDeviceToDevice, s));
     }
-    *out = e;
+    k_elastic_cost<<<(estride + ELASTIC_COLS - 1) / ELASTIC_COLS, ELASTIC_COLS, 0, s>>>(W, tiles, a);
+    ctx->launches += 1;
+    CK(cudaGetLastError());
+    int crashed = 0;  // *n_crashed stays 0 unless the call succeeds
+    CK(cudaMemcpyAsync(&crashed, a.count, sizeof(int), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    *n_crashed = crashed;
+    *out = e.release();
     return JSLP_OK;
 }

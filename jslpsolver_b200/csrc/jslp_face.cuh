@@ -98,14 +98,33 @@ __global__ void __launch_bounds__(FACE_TILE * FACE_TILE) k_face_gather(const Tab
 
 }  // namespace jslp
 
-// What a sibling tab (jslp_face_create, jslp_bound_create) takes over from its parent besides the tableau: the
-// unrestricted / integer tables over labels [0, n_index) and every jslp_tab_set_option value.  n_index >= the
-// parent's; the labels from the parent's n_index on are restricted and not integer.  The element indices stay the
-// parent's, so a label means the same in both tabs.
-static int inherit_tables_and_options(const jslp_tab *t, jslp_tab *f, int n_index) {
+// Owners for what a builder allocates: CK returns early, and a half-built sibling must not outlive the call.
+struct TabDestroy { void operator()(jslp_tab *t) const { jslp_tab_destroy(t); } };
+struct DevFree { void operator()(void *p) const { cudaFree(p); } };
+using TabOwner = std::unique_ptr<jslp_tab, TabDestroy>;
+
+// l* = max(n_index, lastElementIndex): the first label neither the label tables nor the cut rows have handed out.
+static int first_free_label(const jslp_tab *t) { return std::max(t->n_index, t->lastElementIndex); }
+
+// A sibling tab of t (jslp_face_create, jslp_bound_create, jslp_elastic_create, jslp_cone_create), W x H in the same
+// context, with row capacity max(t's, H).  With new_labels == 0 it has t's labels (nVars, lastElementIndex, n_index);
+// otherwise new_labels more, l*..l*+new_labels-1: nVars + new_labels and lastElementIndex = n_index = l* + new_labels,
+// so cut rows would take labels after them.  It takes over the unrestricted / integer tables over labels [0, n_index)
+// (the new labels restricted and not integer) and every jslp_tab_set_option value, and its descriptor is on the
+// device.  The element indices stay the parent's, so a label means the same in both tabs.
+static int sibling_create(const jslp_tab *t, int W, int H, int new_labels, TabOwner &child) {
+    jslp_tab *f = nullptr;
+    int rc = jslp_tab_create(t->ctx, W, H, std::max(t->rowcap, H), t->precision, &f);
+    if (rc) return rc;
+    child.reset(f);
+    if (new_labels == 0) {
+        f->nVars = t->nVars; f->lastElementIndex = t->lastElementIndex; f->n_index = t->n_index;
+    } else {
+        const int label = first_free_label(t);
+        f->nVars = t->nVars + new_labels; f->lastElementIndex = label + new_labels; f->n_index = label + new_labels;
+    }
     cudaStream_t s = t->ctx->stream;
-    const size_t n0 = (size_t)t->n_index, n1 = (size_t)n_index;
-    f->n_index = n_index;
+    const size_t n0 = (size_t)t->n_index, n1 = (size_t)f->n_index;
     if (t->hd.unres) {
         CK(cudaMalloc(&f->hd.unres, n1));
         if (n1 > n0) CK(cudaMemsetAsync(f->hd.unres + n0, 0, n1 - n0, s));
@@ -123,7 +142,7 @@ static int inherit_tables_and_options(const jslp_tab *t, jslp_tab *f, int n_inde
     f->timeline_cap = t->timeline_cap; f->pdl = t->pdl; f->pingpong = t->pingpong;
     f->node_slots = t->node_slots; f->node_log_cap = t->node_log_cap; f->slot_steps = t->slot_steps;
     f->slot_variant = t->slot_variant; f->use_mir = t->use_mir;
-    return JSLP_OK;
+    return push_desc(f);
 }
 
 // The face of t into *face (nullptr when only column 0 is kept).  With d_cost (a device array of C by label) row 0 is
@@ -135,52 +154,37 @@ static int face_build(jslp_tab *t, const double *d_cost, jslp_tab **face, int32_
     const int W = t->W, H = t->H;
     int *d_plan = nullptr;  // map[W], vcol'[W], W'
     CK(cudaMalloc(&d_plan, sizeof(int) * (2 * (size_t)W + 1)));
+    const std::unique_ptr<int, DevFree> plan(d_plan);
     int *d_map = d_plan, *d_vcol = d_plan + W, *d_n = d_plan + 2 * (size_t)W;
-    jslp_tab *f = nullptr;
-    int rc = JSLP_OK, Wk = 0;
-    // CK returns: release what this call owns on the way out
-    auto body = [&]() -> int {
-        k_face_plan<<<1, FACE_PLAN_THREADS, 0, s>>>(t->d_T, d_map, d_vcol, d_n);
-        ctx->launches += 1;
-        CK(cudaGetLastError());
-        CK(cudaMemcpyAsync(&Wk, d_n, sizeof(int), cudaMemcpyDeviceToHost, s));
+    int Wk = 0;
+    k_face_plan<<<1, FACE_PLAN_THREADS, 0, s>>>(t->d_T, d_map, d_vcol, d_n);
+    ctx->launches += 1;
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(&Wk, d_n, sizeof(int), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    if (Wk < 1 || Wk > W) return fail(JSLP_E_CUDA, "face_create: the plan kernel returned a bad column count");
+    *n_keep = Wk;
+    if (kept_cols) {
+        CK(cudaMemcpyAsync(kept_cols, d_map, sizeof(int) * (size_t)Wk, cudaMemcpyDeviceToHost, s));
         CK(cudaStreamSynchronize(s));
-        if (Wk < 1 || Wk > W) return fail(JSLP_E_CUDA, "face_create: the plan kernel returned a bad column count");
-        *n_keep = Wk;
-        if (kept_cols) {
-            CK(cudaMemcpyAsync(kept_cols, d_map, sizeof(int) * (size_t)Wk, cudaMemcpyDeviceToHost, s));
-            CK(cudaStreamSynchronize(s));
-        }
-        if (Wk == 1) return JSLP_OK;  // nothing but column 0: the optimum is the only point of the face
-        int rc2 = jslp_tab_create(ctx, Wk, H, t->rowcap, t->precision, &f);
-        if (rc2) return rc2;
-        // labels, tables and options of the parent
-        f->nVars = t->nVars; f->lastElementIndex = t->lastElementIndex;
-        rc2 = inherit_tables_and_options(t, f, t->n_index);
-        if (rc2) return rc2;
-        rc2 = push_desc(f);
-        if (rc2) return rc2;
-        CK(cudaMemcpyAsync(f->hd.vcol, d_vcol, sizeof(int) * (size_t)Wk, cudaMemcpyDeviceToDevice, s));
-        const dim3 grid((unsigned)(f->stride / FACE_TILE), (unsigned)((H + FACE_ROWS - 1) / FACE_ROWS));
-        k_face_gather<<<grid, FACE_TILE * FACE_TILE, 0, s>>>(t->d_T, d_map, Wk, f->hd.M, f->stride, f->hd.vrow);
-        ctx->launches += 1;
-        CK(cudaGetLastError());
-        if (d_cost) {  // over the +0 the gather wrote at the kept columns; the padding stays +0
-            k_price_objective<<<(Wk + FR_COLS - 1) / FR_COLS, FR_COLS, 0, s>>>(t->d_T, d_cost, d_map, Wk, f->hd.M,
-                                                                               nullptr);
-            ctx->launches += 1;
-            CK(cudaGetLastError());
-        }
-        CK(cudaStreamSynchronize(s));
-        return JSLP_OK;
-    };
-    rc = body();
-    cudaFree(d_plan);
-    if (rc) {
-        if (f) jslp_tab_destroy(f);
-        return rc;
     }
-    *face = f;
+    if (Wk == 1) return JSLP_OK;  // nothing but column 0: the optimum is the only point of the face
+    TabOwner f;
+    const int rc = sibling_create(t, Wk, H, 0, f);
+    if (rc) return rc;
+    CK(cudaMemcpyAsync(f->hd.vcol, d_vcol, sizeof(int) * (size_t)Wk, cudaMemcpyDeviceToDevice, s));
+    const dim3 grid((unsigned)(f->stride / FACE_TILE), (unsigned)((H + FACE_ROWS - 1) / FACE_ROWS));
+    k_face_gather<<<grid, FACE_TILE * FACE_TILE, 0, s>>>(t->d_T, d_map, Wk, f->hd.M, f->stride, f->hd.vrow);
+    ctx->launches += 1;
+    CK(cudaGetLastError());
+    if (d_cost) {  // over the +0 the gather wrote at the kept columns; the padding stays +0
+        k_price_objective<<<(Wk + FR_COLS - 1) / FR_COLS, FR_COLS, 0, s>>>(t->d_T, d_cost, d_map, Wk, f->hd.M,
+                                                                           nullptr);
+        ctx->launches += 1;
+        CK(cudaGetLastError());
+    }
+    CK(cudaStreamSynchronize(s));
+    *face = f.release();
     return JSLP_OK;
 }
 

@@ -13,20 +13,9 @@
 
 enum { SCEN_OPTIMAL = 0, SCEN_INFEASIBLE = 1, SCEN_UNBOUNDED = 2, SCEN_CYCLED = 3 };
 
-static int scen_scratch(jslp_tab *t, size_t bytes) {
-    if (bytes <= t->scen_bytes) return JSLP_OK;
-    cudaFree(t->d_scen);
-    t->d_scen = nullptr;
-    t->scen_bytes = 0;
-    CK(cudaMalloc(&t->d_scen, bytes));
-    t->scen_bytes = bytes;
-    return JSLP_OK;
-}
-
 // One scenario on the single-tableau path, from the private snapshot.
 static int scenario_sequential(jslp_tab *t, const jslp_scenario_edit *e, int n, int check_cycles, int32_t *status,
                                double *eval_raw, int32_t *p1, int32_t *p2, double *rhs, int32_t *vrow) {
-    cudaStream_t s = t->ctx->stream;
     int rc = snapshot_copy(t, 2, false);
     for (int k = 0; k < n && rc == JSLP_OK; k++)
         rc = e[k].kind == 0 ? jslp_update_rhs(t, e[k].index, e[k].difference)
@@ -39,11 +28,7 @@ static int scenario_sequential(jslp_tab *t, const jslp_scenario_edit *e, int n, 
     *eval_raw = st.evaluation_raw;
     *p1 = st.phase1_pivots;
     *p2 = st.phase2_pivots;
-    CK(cudaMemcpy2DAsync(rhs, sizeof(double), t->hd.M, sizeof(double) * t->stride, sizeof(double), t->H,
-                         cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(vrow, t->hd.vrow, sizeof(int) * (size_t)t->H, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    return JSLP_OK;
+    return read_column(t, 0, rhs, vrow);
 }
 
 // Scenarios [s0, s0 + n) in one k_node_batch<NODE_SCENARIO> launch.  Those whose log shows a cycle (per-phase
@@ -51,63 +36,43 @@ static int scenario_sequential(jslp_tab *t, const jslp_scenario_edit *e, int n, 
 static int scenario_resident(jslp_tab *t, const std::vector<EditDev> &res, const int32_t *offsets, int s0, int n,
                              int check_cycles, int32_t *status, double *eval_raw, int32_t *p1, int32_t *p2,
                              double *rhs, int32_t *vrow, std::vector<int> &redo) {
-    jslp_ctx *ctx = t->ctx;
-    cudaStream_t s = ctx->stream;
     ResidentBufs &rb = t->rbufs;
     const int H0 = t->H;
-    int Ws = 0;
-    const size_t smem = node_smem_bytes(H0, t->W, &Ws);
-    const int log_cap = t->node_log_cap;
-    int rc = rb.ensure(n, 0, log_cap);
+    const Snapshot &src = t->snaps[2];
+    NodeBatchDev nb;
+    size_t smem = 0;
+    int rc = batch_fill(t, src.M, src.vrow, src.vcol, H0, t->lastElementIndex, n, nb, &smem);
     if (rc) return rc;
     // one device block per chunk: offsets, edits, final columns, final labels
     const int e0 = offsets[s0], ne = offsets[s0 + n] - e0;
     const size_t b_off = 0, b_ed = (sizeof(int) * (size_t)(n + 1) + 15) & ~(size_t)15;
     const size_t b_rhs = b_ed + sizeof(EditDev) * (size_t)ne;
     const size_t b_vrow = b_rhs + sizeof(double) * (size_t)n * H0;
-    rc = scen_scratch(t, b_vrow + sizeof(int) * (size_t)n * H0);
+    rc = batch_scratch(t, b_vrow + sizeof(int) * (size_t)n * H0);
     if (rc) return rc;
-    char *base = (char *)t->d_scen;
+    char *base = (char *)t->d_scratch;
     std::vector<int> off((size_t)n + 1);
     for (int i = 0; i <= n; i++) off[i] = offsets[s0 + i] - e0;
+    cudaStream_t s = t->ctx->stream;
     CK(cudaMemcpyAsync(base + b_off, off.data(), sizeof(int) * (size_t)(n + 1), cudaMemcpyHostToDevice, s));
     if (ne > 0) CK(cudaMemcpyAsync(base + b_ed, res.data() + e0, sizeof(EditDev) * (size_t)ne, cudaMemcpyHostToDevice, s));
-    NodeBatchDev nb;
-    memset(&nb, 0, sizeof(nb));
-    const Snapshot &src = t->snaps[2];
-    nb.rootM = src.M; nb.root_vrow = src.vrow; nb.root_vcol = src.vcol;
-    nb.cut_off = (const int *)(base + b_off); nb.out = rb.dv_out; nb.logs = rb.d_logs;
-    nb.H0 = H0; nb.root_stride = t->stride; nb.first_index = t->lastElementIndex;
-    nb.Hcap = H0; nb.Ws = Ws; nb.log_cap = log_cap; nb.max_pivots = 100000;
+    nb.cut_off = (const int *)(base + b_off);
     nb.edits = (const EditDev *)(base + b_ed);
     nb.out_rhs = (double *)(base + b_rhs); nb.out_vrow = (int *)(base + b_vrow);
     if (n <= NODE_INLINE_OFF) {
         nb.n_inline = n;
         for (int i = 0; i <= n; i++) nb.cut_off_inline[i] = off[i];
     }
-    CK(cudaFuncSetAttribute(k_node_batch<NODE_SCENARIO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k_node_batch<NODE_SCENARIO><<<n, NODE_THREADS, smem, s>>>(t->d_T, nb);
-    ctx->launches += 1;
-    CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(rhs + (size_t)s0 * H0, nb.out_rhs, sizeof(double) * (size_t)n * H0, cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(vrow + (size_t)s0 * H0, nb.out_vrow, sizeof(int) * (size_t)n * H0, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
+    rc = batch_launch<NODE_SCENARIO>(t, nb, n, smem, rhs + (size_t)s0 * H0, vrow + (size_t)s0 * H0);
+    if (rc) return rc;
     bool need_full = false;
     for (int i = 0; i < n; i++) need_full |= check_cycles && !rb.h_out[i].r.overflow && rb.h_out[i].r.log_n > NODE_LOG_HEAD;
-    if (need_full) {
-        CK(cudaMemcpyAsync(rb.h_logs, rb.d_logs, sizeof(int4) * (size_t)n * log_cap, cudaMemcpyDeviceToHost, s));
-        CK(cudaStreamSynchronize(s));
-    }
+    rc = batch_fetch_logs(t, n, need_full);
+    if (rc) return rc;
     for (int i = 0; i < n; i++) {
         const NodeResult &r = rb.h_out[i].r;
-        bool again = r.overflow != 0;
-        if (!again && check_cycles) {
-            CycleHist h[2];  // (leaving, entering) per phase (simplex.ts:27,102)
-            int cs, cl;
-            const int4 *lg = r.log_n > NODE_LOG_HEAD ? rb.h_logs + (size_t)i * log_cap : rb.h_out[i].log_head;
-            for (int k = 0; k < r.log_n && k < log_cap && !again; k++)
-                again = h[((lg[k].x >> 30) & 1) ? 1 : 0].push_and_check(((long long)lg[k].z << 32) | (unsigned int)lg[k].w, &cs, &cl);
-        }
+        const bool again =
+            r.overflow || (check_cycles && first_cycle(batch_log(t, i), std::min(r.log_n, t->node_log_cap)) >= 0);
         if (again) { redo.push_back(s0 + i); continue; }
         status[s0 + i] = r.status == ST_OPTIMAL ? SCEN_OPTIMAL : r.status == ST_UNBOUNDED ? SCEN_UNBOUNDED : SCEN_INFEASIBLE;
         eval_raw[s0 + i] = r.eval_raw;
@@ -148,18 +113,14 @@ extern "C" int jslp_scenario_batch(jslp_tab *t, const jslp_scenario_edit *edits,
             if (e.kind == 0) res[k] = row < 0 ? EditDev{EDIT_RHS_COL, col, e.difference} : EditDev{EDIT_RHS_ROW, row, e.difference};
             else res[k] = row < 0 ? EditDev{EDIT_COST_COL, col, e.difference} : EditDev{EDIT_COST_ROW, row, e.difference};
         }
-    // the scalar Tableau state and the executed-pivot log describe the caller's tableau, not these scenarios
-    const int feasible = t->feasible, bounded = t->bounded, iters = t->simplexIters, unb = t->unboundedVar;
-    const double evaluation = t->evaluation, best = t->bestPossibleEval;
-    const size_t log_size = t->host_log.size();
+    const CallerState caller(t);
     rc = ensure_snapshot(t, 2);
     if (rc) return rc;
     rc = snapshot_copy(t, 2, true);
     if (rc) return rc;
     std::vector<int> redo;
-    if (t->engine != 1 && t->engine != 2 && resident_fits(t, t->H)) {
-        // chunks keep the per-scenario outputs on the device bounded (about 32 MB)
-        const int chunk = (int)std::max<size_t>(1, std::min<size_t>(4096, ((size_t)32 << 20) / ((size_t)12 * t->H)));
+    if (batch_resident(t, t->H)) {
+        const int chunk = batch_chunk(t->H);
         for (int s0 = 0; s0 < n_scenarios && rc == JSLP_OK; s0 += chunk)
             rc = scenario_resident(t, res, offsets, s0, std::min(chunk, n_scenarios - s0), check_cycles, status, eval_raw,
                                    p1, p2, rhs, vrow, redo);
@@ -176,8 +137,6 @@ extern "C" int jslp_scenario_batch(jslp_tab *t, const jslp_scenario_edit *edits,
     const int rc2 = snapshot_copy(t, 2, false);
     if (rc == JSLP_OK) rc = rc2;
     CK(cudaStreamSynchronize(t->ctx->stream));
-    t->feasible = feasible; t->bounded = bounded; t->simplexIters = iters; t->unboundedVar = unb;
-    t->evaluation = evaluation; t->bestPossibleEval = best;
-    if (t->host_log.size() > log_size) t->host_log.resize(log_size);
+    caller.restore(t);
     return rc;
 }

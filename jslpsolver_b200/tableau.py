@@ -733,6 +733,18 @@ class GpuTableau:
             p2.ctypes.data, rhs.ctypes.data, vrow.ctypes.data))
         return {"status": status, "eval_raw": eval_raw, "p1": p1, "p2": p2, "rhs": rhs, "vrow": vrow}
 
+    def _adopt(self, h) -> "GpuTableau":
+        """A GpuTableau over the tab handle h that the library derived from this one (face, bound, lex_next, elastic,
+        cone): this tableau's precision, context, model, integer count, engine and options, no optional objectives,
+        and its size and labels as the library set them."""
+        c = GpuTableau(self.precision, context=self.context)
+        c.handle = h
+        c.model, c.variablesPerIndex = self.model, self.variablesPerIndex
+        c.nOpt, c.nInts = 0, getattr(self, "nInts", 0)
+        c.engine, c.options = self.engine, dict(self.options)
+        c._refresh_dims()
+        return c
+
     def face(self):
         """jslp_face_create: (face, kept columns).  `face` is a GpuTableau of the optimal face of the current (optimal)
         tableau -- the columns whose cost entry lies within the precision, under a zero cost row, with this
@@ -745,13 +757,7 @@ class GpuTableau:
         kept = kept[:n.value].copy()
         if not h.value:
             return None, kept
-        f = GpuTableau(self.precision, context=self.context)
-        f.handle = h
-        f.model, f.variablesPerIndex = self.model, self.variablesPerIndex
-        f.width, f.height = n.value, self.height
-        f.nVars, f.lastElementIndex, f.nOpt, f.nInts = self.nVars, self.lastElementIndex, 0, getattr(self, "nInts", 0)
-        f.engine, f.options = self.engine, dict(self.options)
-        return f, kept
+        return self._adopt(h), kept
 
     def bound(self, allowance: float) -> "GpuTableau":
         """jslp_bound_create: a GpuTableau of the current (optimal) tableau with its objective turned into one bound
@@ -762,13 +768,7 @@ class GpuTableau:
         L = self.context.lib
         h = C.c_void_p()
         _lib.check(L.jslp_bound_create(self._h(), float(allowance), C.byref(h)))
-        b = GpuTableau(self.precision, context=self.context)
-        b.handle = h
-        b.model, b.variablesPerIndex = self.model, self.variablesPerIndex
-        b.nOpt, b.nInts = 0, getattr(self, "nInts", 0)
-        b.engine, b.options = self.engine, dict(self.options)
-        b._refresh_dims()
-        return b
+        return self._adopt(h)
 
     def lex_next(self, cost_by_label, allowance: float):
         """jslp_lex_next: (next, kept columns).  `next` is the starting tableau of the next level of a lexicographic
@@ -787,13 +787,7 @@ class GpuTableau:
         kept = kept[:n.value].copy()
         if not h.value:
             return None, kept
-        f = GpuTableau(self.precision, context=self.context)
-        f.handle = h
-        f.model, f.variablesPerIndex = self.model, self.variablesPerIndex
-        f.nOpt, f.nInts = 0, getattr(self, "nInts", 0)
-        f.engine, f.options = self.engine, dict(self.options)
-        f._refresh_dims()
-        return f, kept
+        return self._adopt(h), kept
 
     def elastic(self, rows, weights):
         """jslp_elastic_create: (elastic, crashed).  `elastic` is a GpuTableau of this tableau, as upload() left it,
@@ -809,13 +803,7 @@ class GpuTableau:
         _lib.check(self.context.lib.jslp_elastic_create(self._h(), r.ctypes.data if len(r) else None,
                                                         w.ctypes.data if len(w) else None, len(r), C.byref(h),
                                                         C.byref(n)))
-        e = GpuTableau(self.precision, context=self.context)
-        e.handle = h
-        e.model, e.variablesPerIndex = self.model, self.variablesPerIndex
-        e.nOpt, e.nInts = 0, getattr(self, "nInts", 0)
-        e.engine, e.options = self.engine, dict(self.options)
-        e._refresh_dims()
-        return e, n.value
+        return self._adopt(h), n.value
 
     def cone(self) -> "GpuTableau":
         """jslp_cone_create: a GpuTableau of the recession cone of this tableau, as upload() left it -- column 0 set to
@@ -824,13 +812,7 @@ class GpuTableau:
         this tableau is only read.  close() it when done."""
         h = C.c_void_p()
         _lib.check(self.context.lib.jslp_cone_create(self._h(), C.byref(h)))
-        k = GpuTableau(self.precision, context=self.context)
-        k.handle = h
-        k.model, k.variablesPerIndex = self.model, self.variablesPerIndex
-        k.nOpt, k.nInts = 0, getattr(self, "nInts", 0)
-        k.engine, k.options = self.engine, dict(self.options)
-        k._refresh_dims()
-        return k
+        return self._adopt(h)
 
     def column_batch(self, keep_cols) -> dict:
         """jslp_column_batch: simplex() (cycle check on) of the saved snapshot with the columns not kept in keep[s]
