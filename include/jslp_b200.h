@@ -355,6 +355,34 @@ int jslp_cone_create(jslp_tab *tab, jslp_tab **cone);
 int jslp_column_batch(jslp_tab *tab, const uint8_t *keep_cols, int n_sets, int32_t *status, double *eval_raw,
                       int32_t *pivots, double *rhs, int32_t *vrow);
 
+/* One fixing of a solution-pool region: the non-basic column `column` (1..W-1) of the snapshot held at `value`. */
+typedef struct {
+    int32_t column;
+    double value;
+} jslp_fix;
+
+/* The region LPs of a MIP solution-pool search, DESIGN.md section 2m.  Region i is the saved snapshot (the model's
+ * initial tableau) with fixes[fix_offsets[i] .. fix_offsets[i+1]) applied in order -- M[r,0] = M[r,0] - value *
+ * M[r,column], then M[r,column] = +0, for every row r, row 0 included -- then the cut rows cuts[cut_offsets[i] ..
+ * cut_offsets[i+1]) appended as jslp_add_cuts appends them (labels from the snapshot's lastElementIndex), then
+ * simplex() with check_cycles and the isIntegral / getMostFractionalVar scan.  Regions whose rows fit shared memory
+ * run one CTA each in one launch; the others, and any region whose pivot log shows a cycle or that hits the in-kernel
+ * pivot or log cap, run one after another on the single-tableau path.  Per region:
+ *   status         0 optimal, 1 infeasible, 2 unbounded, 3 cycled (the cycle check fired)
+ *   evaluation     Tableau.evaluation when optimal (M[0,0] rounded to the precision), -inf when unbounded, else 0
+ *   is_integral    1 when optimal and every basic integer variable is integral
+ *   branch_var / branch_value   getMostFractionalVar when optimal and not integral, else -1 / 0
+ *   pivots         phase-1 plus phase-2 pivots
+ *   rhs, vrow      row_stride entries each at i * row_stride; for an integral region the first H + n_cuts(i) hold the
+ *                  final column 0 and row labels, otherwise they are not written
+ * row_stride must be at least the snapshot's height plus every region's cut count.  Needs a snapshot (jslp_save); on
+ * return the tableau equals it, and the scalar Tableau state and executed-pivot log are as they were.  No optional
+ * objectives (JSLP_E_UNSUPPORTED). */
+int jslp_pool_batch(jslp_tab *tab, const jslp_fix *fixes, const int32_t *fix_offsets, const jslp_cut *cuts,
+                    const int32_t *cut_offsets, int n_nodes, int check_cycles, int row_stride, int32_t *status,
+                    double *evaluation, int32_t *is_integral, int32_t *branch_var, double *branch_value,
+                    int32_t *pivots, double *rhs, int32_t *vrow);
+
 /* Column `col` (0..W-1) of the current tableau, H doubles, into out: one strided device-to-host copy, so a single
  * column of a large tableau is read without downloading the whole of it. */
 int jslp_column(jslp_tab *tab, int col, double *out);

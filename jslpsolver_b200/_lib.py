@@ -35,6 +35,10 @@ class ScenarioEdit(C.Structure):  # jslp_scenario_edit
     _fields_ = [("kind", C.c_int32), ("index", C.c_int32), ("difference", C.c_double)]
 
 
+class Fix(C.Structure):  # jslp_fix
+    _fields_ = [("column", C.c_int32), ("value", C.c_double)]
+
+
 ALL_GATHER_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_int64)
 
 
@@ -114,6 +118,7 @@ SYMBOLS = [
     ("jslp_cone_create", C.c_int, [P, C.POINTER(P)]),
     ("jslp_column_batch", C.c_int, [P, P, C.c_int, P, P, P, P, P]),
     ("jslp_column", C.c_int, [P, C.c_int, P]),
+    ("jslp_pool_batch", C.c_int, [P, P, P, P, P, C.c_int, C.c_int, C.c_int, P, P, P, P, P, P, P, P]),
     ("jslp_branch_and_cut", C.c_int, [P, C.POINTER(BnbOpts), C.POINTER(BnbStatus), P, C.c_int]),
     ("jslp_bnb_node_log", C.c_int, [P, P, C.c_int64, C.POINTER(C.c_int64)]),
     ("jslp_bnb_solution", C.c_int, [P, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_int32), P, P, C.c_int]),

@@ -81,7 +81,7 @@ static int batch_fill(jslp_tab *t, const double *M, const int *vrow, const int *
     return JSLP_OK;
 }
 
-// One k_node_batch<MODE> launch of n sets; with out_rhs set, the final columns and labels to rhs / vrow (n x H0).
+// One k_node_batch<MODE> launch of n sets; with out_rhs set, the final columns and labels to rhs / vrow (n x Hcap).
 template <int MODE>
 static int batch_launch(jslp_tab *t, const NodeBatchDev &nb, int n, size_t smem, double *rhs, int32_t *vrow) {
     jslp_ctx *ctx = t->ctx;
@@ -91,8 +91,8 @@ static int batch_launch(jslp_tab *t, const NodeBatchDev &nb, int n, size_t smem,
     ctx->launches += 1;
     CK(cudaGetLastError());
     if (nb.out_rhs) {
-        CK(cudaMemcpyAsync(rhs, nb.out_rhs, sizeof(double) * (size_t)n * nb.H0, cudaMemcpyDeviceToHost, s));
-        CK(cudaMemcpyAsync(vrow, nb.out_vrow, sizeof(int) * (size_t)n * nb.H0, cudaMemcpyDeviceToHost, s));
+        CK(cudaMemcpyAsync(rhs, nb.out_rhs, sizeof(double) * (size_t)n * nb.Hcap, cudaMemcpyDeviceToHost, s));
+        CK(cudaMemcpyAsync(vrow, nb.out_vrow, sizeof(int) * (size_t)n * nb.Hcap, cudaMemcpyDeviceToHost, s));
     }
     CK(cudaStreamSynchronize(s));
     return JSLP_OK;

@@ -45,6 +45,7 @@ enum NodeMode : int {
     NODE_SUBSET = 1,    // one row subset of the root per CTA (jslp_feasibility_batch)
     NODE_SCENARIO = 2,  // one list of right-hand-side / cost edits of the root per CTA (jslp_scenario_batch)
     NODE_COLUMNS = 3,   // one column subset of the root per CTA, the others zeroed (jslp_column_batch)
+    NODE_POOL = 4,      // one region of a solution-pool search per CTA: fixed columns, then cut rows (jslp_pool_batch)
 };
 
 // One resolved scenario edit (DESIGN.md 2e): where updateRightHandSide / updateCost (dynamic-modification.ts:78-160)
@@ -54,6 +55,8 @@ enum EditKind : int {
     EDIT_RHS_ROW = 1,   // slack basic in row pos: M[pos,0] -= d
     EDIT_COST_ROW = 2,  // variable basic in row pos: M[0,c] += d * M[pos,c] for every column, column 0 included
     EDIT_COST_COL = 3,  // variable non-basic in column pos: M[0,pos] -= d
+    EDIT_FIX_COL = 4,   // variable non-basic in column pos held at d (DESIGN.md 2m): M[r,0] -= d * M[r,pos], then
+                        // M[r,pos] = +0, for every row, row 0 included
 };
 struct EditDev {
     int kind, pos;
@@ -79,9 +82,13 @@ struct NodeBatchDev {
     int keep_words, phase1_only;
     // scenario launches (NODE_SCENARIO, jslp_scenario_batch): node n applies edits[cut_off[n] .. cut_off[n+1]) (device
     // memory; every right-hand-side edit before every cost edit) to the restored root, solves, and writes its final
-    // column 0 and row labels to out_rhs / out_vrow + n * H0 (NODE_COLUMNS writes them too).  Not read by the other
+    // column 0 and row labels to out_rhs / out_vrow + n * Hcap (NODE_COLUMNS writes them too).  Not read by the other
     // modes.
+    // Pool launches (NODE_POOL, jslp_pool_batch) apply the EDIT_FIX_COL edits[edit_off[n] .. edit_off[n+1]) (device
+    // memory) to the restored root in list order, then append node n's cut rows as NODE_BRANCH does; they write column
+    // 0 and the row labels too.  The final columns go to out_rhs / out_vrow + n * Hcap.
     const EditDev *edits;
+    const int *edit_off;
     double *out_rhs;
     int *out_vrow;
     int n_inline;         // > 0: cut_off_inline holds the n_inline + 1 offsets (saves a PCIe round trip)
@@ -147,11 +154,13 @@ struct NodePart {    // per-warp partial results of a scan
 // subset of the root per CTA (NodeBatchDev.keep), compacted in row order; row labels stay the root's, so the
 // unrestricted lookup and the pivot log read as on the whole tableau.  NODE_SCENARIO: every root row, then the CTA's
 // edit list applied to column 0 and row 0 (DESIGN.md 2e) in place of cut rows.  NODE_COLUMNS: every root row, with the
-// columns cleared in the CTA's mask set to +0 in every row, row 0 included (DESIGN.md 2l).  A template parameter, so
-// that the node path carries none of the subset, scenario or column code.
+// columns cleared in the CTA's mask set to +0 in every row, row 0 included (DESIGN.md 2l).  NODE_POOL: every root row,
+// the CTA's fixings applied by the scenario edit loop, then its cut rows (DESIGN.md 2m).  A template parameter, so
+// that the node path carries none of the subset, scenario, column or pool code.
 template <int MODE>
 __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, const __grid_constant__ NodeBatchDev nb) {
     constexpr bool SUBSET = MODE == NODE_SUBSET, SCENARIO = MODE == NODE_SCENARIO, COLUMNS = MODE == NODE_COLUMNS;
+    constexpr bool POOL = MODE == NODE_POOL;
     extern __shared__ __align__(16) unsigned char smraw[];
     __shared__ TabDev T;
     __shared__ SelSmem sel;
@@ -233,22 +242,29 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
     if (SUBSET)  // nobody reads slot until the barrier after the cut rows
         for (int r = tid; r < nb.Hcap; r += NT) slot[r] = r;
     if (tid == 0) tl1 = globaltimer_ns() - t_start;
-    if constexpr (SCENARIO) {
+    if constexpr (SCENARIO || POOL) {
         // setRightHandSide / setCost on the restored root (DESIGN.md 2e): every edit writes column 0 or row 0 only and
         // reads columns >= 1 / rows >= 1, so the right-hand-side edits run as one pass over rows (each thread applies
-        // all of them to its M[r,0] in order) and the cost edits, after them, as one pass over columns.
-        const EditDev *ed = nb.edits + c0;
-        for (int r = tid; r < Hn; r += NT) {
+        // all of them to its M[r,0] in order) and the cost edits, after them, as one pass over columns.  A fixing
+        // (DESIGN.md 2m) reads and then clears its own column of the thread's row, so it joins the row pass.
+        int e0 = c0, ne = nc;
+        if constexpr (POOL) { e0 = nb.edit_off[node]; ne = nb.edit_off[node + 1] - e0; }
+        const EditDev *ed = nb.edits + e0;
+        for (int r = tid; r < H0k; r += NT) {
             double *row = Ms + (size_t)r * Ws;
             double x = row[0];
-            for (int k = 0; k < nc; k++) {
+            for (int k = 0; k < ne; k++) {
                 const EditDev e = ed[k];
                 if (e.kind == EDIT_RHS_COL) x = edit_axpy_sub(x, e.d, row[e.pos]);
                 else if (e.kind == EDIT_RHS_ROW && e.pos == r) x = edit_sub(x, e.d);
+                else if (POOL && e.kind == EDIT_FIX_COL) { x = edit_axpy_sub(x, e.d, row[e.pos]); row[e.pos] = 0.0; }
             }
             row[0] = x;
         }
         __syncthreads();
+    }
+    if constexpr (SCENARIO) {
+        const EditDev *ed = nb.edits + c0;
         for (int c = tid; c < W; c += NT) {
             double x = Ms[c];
             for (int k = 0; k < nc; k++) {
@@ -499,10 +515,10 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
     // isIntegral / most fractional variable over the final RHS column
     for (int r = tid; r < Hn; r += NT) rhs[r] = Ms[(size_t)slot[r] * Ws];
     __syncthreads();
-    if constexpr (SCENARIO || COLUMNS)
+    if constexpr (SCENARIO || COLUMNS || POOL)
         for (int r = tid; r < Hn; r += NT) {
-            nb.out_rhs[(size_t)node * H0 + r] = rhs[r];
-            nb.out_vrow[(size_t)node * H0 + r] = vrow[r];
+            nb.out_rhs[(size_t)node * nb.Hcap + r] = rhs[r];
+            nb.out_vrow[(size_t)node * nb.Hcap + r] = vrow[r];
         }
     if (T.intpos != nullptr) {
         if (tid == 0) { T.M = rhs; T.stride = 1; T.vrow = vrow; T.H = Hn; }

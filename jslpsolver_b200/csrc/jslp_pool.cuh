@@ -1,0 +1,219 @@
+// jslpsolver_b200/csrc/jslp_pool.cuh -- the region LPs of a MIP solution-pool search (included by jslp_api.cu after
+// jslp_cone.cuh; no reference counterpart).  DESIGN.md section 2m is the contract; in short, with M the saved snapshot
+// (the model's initial tableau, every structural column non-basic), region i is
+//
+//   M with the fixings of i applied in list order -- M[r,0] = M[r,0] - v * M[r,j], then M[r,j] = +0, for every row r,
+//   row 0 included -- followed by the cut rows of i as addCutConstraints builds them, then simplex() with the cycle
+//   check as asked, then the isIntegral / getMostFractionalVar scan.
+//
+// Regions whose rows fit shared memory run one CTA each in k_node_batch<NODE_POOL> (the fixings ride the scenario edit
+// loop as EDIT_FIX_COL edits); the others, and any region whose log shows a cycle or that hits the in-kernel pivot or
+// log cap, run one after another on the single-tableau path: jslp_restore, k_fix_columns, jslp_add_cuts, run_lp,
+// mip_scan.  Both apply the fixings with the same arithmetic in the same order.
+#pragma once
+
+namespace jslp {
+
+// The fixings of one region on the current buffer (the single-tableau path of jslp_pool_batch): one thread per row,
+// each fixing in list order, the arithmetic of k_node_batch<NODE_POOL>'s edit loop.
+__global__ void __launch_bounds__(256) k_fix_columns(const TabDev *Tp, const EditDev *fixes, int n) {
+    const TabDev &T = *Tp;
+    const int r = blockIdx.x * 256 + threadIdx.x;
+    if (r >= T.H) return;
+    double *row = T.M + (size_t)r * T.stride;
+    double x = row[0];
+    for (int k = 0; k < n; k++) {
+        const EditDev e = fixes[k];
+        x = edit_axpy_sub(x, e.d, row[e.pos]);
+        row[e.pos] = 0.0;
+    }
+    row[0] = x;
+}
+
+}  // namespace jslp
+
+enum { POOL_OPTIMAL = 0, POOL_INFEASIBLE = 1, POOL_UNBOUNDED = 2, POOL_CYCLED = 3 };
+
+// What jslp_pool_batch hands back per region, and where.
+struct PoolOut {
+    int32_t *status, *is_integral, *branch_var, *pivots;
+    double *evaluation, *branch_value, *rhs;
+    int32_t *vrow;
+    int row_stride;
+    // the verdict of region i; column 0 and the labels (H entries) are copied by the caller when it is integral
+    void set(int i, int st, double eval_raw, double precision, int integral, int bvar, double bval, int piv) {
+        status[i] = st;
+        evaluation[i] = st == POOL_OPTIMAL ? jslp_round_evaluation(eval_raw, precision) : st == POOL_UNBOUNDED ? -INFINITY : 0.0;
+        is_integral[i] = st == POOL_OPTIMAL ? integral : 0;
+        branch_var[i] = st == POOL_OPTIMAL && !integral ? bvar : -1;
+        branch_value[i] = st == POOL_OPTIMAL && !integral ? bval : 0.0;
+        pivots[i] = piv;
+    }
+};
+
+// One region on the single-tableau path.  The caller restores the snapshot.
+static int pool_hbm(jslp_tab *t, const std::vector<EditDev> &fixes, const jslp_cut *cuts, int n_cuts, int check_cycles,
+                    int i, PoolOut &o) {
+    cudaStream_t s = t->ctx->stream;
+    int rc = jslp_restore(t);
+    if (rc) return rc;
+    if (!fixes.empty()) {
+        rc = batch_scratch(t, sizeof(EditDev) * fixes.size());
+        if (rc) return rc;
+        CK(cudaMemcpyAsync(t->d_scratch, fixes.data(), sizeof(EditDev) * fixes.size(), cudaMemcpyHostToDevice, s));
+        k_fix_columns<<<(t->H + 255) / 256, 256, 0, s>>>(t->d_T, (const EditDev *)t->d_scratch, (int)fixes.size());
+        t->ctx->launches += 1;
+        CK(cudaGetLastError());
+    }
+    rc = jslp_add_cuts(t, cuts, n_cuts);
+    if (rc) return rc;
+    jslp_lp_status st;
+    rc = run_lp(t, 0, check_cycles, &st, false);
+    if (rc) return rc;
+    const int status = st.cycled ? POOL_CYCLED : !st.feasible ? POOL_INFEASIBLE : !st.bounded ? POOL_UNBOUNDED : POOL_OPTIMAL;
+    MipOut mo{};
+    mo.var_index = -1;
+    if (status == POOL_OPTIMAL) {
+        rc = mip_scan(t, &mo);
+        if (rc) return rc;
+    }
+    o.set(i, status, st.evaluation_raw, t->precision, mo.is_integral, mo.var_index, mo.value,
+          st.phase1_pivots + st.phase2_pivots);
+    if (o.is_integral[i]) return read_column(t, 0, o.rhs + (size_t)i * o.row_stride, o.vrow + (size_t)i * o.row_stride);
+    return JSLP_OK;
+}
+
+// Regions idx[0..n) in one k_node_batch<NODE_POOL> launch.  Those whose log shows a cycle (per-phase histories, with
+// check_cycles) or that hit the pivot or log cap go to redo.
+static int pool_resident(jslp_tab *t, const std::vector<EditDev> &fixes, const int32_t *fix_off, const jslp_cut *cuts,
+                         const int32_t *cut_off, const int *idx, int n, int check_cycles, PoolOut &o,
+                         std::vector<int> &redo) {
+    ResidentBufs &rb = t->rbufs;
+    const int H0 = t->saved.H;
+    int maxc = 0, totc = 0, totf = 0;
+    for (int k = 0; k < n; k++) {
+        const int nc = cut_off[idx[k] + 1] - cut_off[idx[k]];
+        maxc = std::max(maxc, nc);
+        totc += nc;
+        totf += fix_off[idx[k] + 1] - fix_off[idx[k]];
+    }
+    int rc = rb.ensure(n, totc, t->node_log_cap);
+    if (rc) return rc;
+    NodeBatchDev nb;
+    size_t smem = 0;
+    rc = batch_fill(t, t->saved.M, t->saved.vrow, t->saved.vcol, H0, t->saved.lastElementIndex, n, nb, &smem);
+    if (rc) return rc;
+    nb.Hcap = H0 + maxc;
+    smem = node_smem_bytes(nb.Hcap, t->W, nullptr);
+    // cut rows: mapped host memory, as branch-and-cut's node launches read them
+    std::vector<int> foff((size_t)n + 1);
+    std::vector<EditDev> fx((size_t)std::max(1, totf));
+    int c = 0, f = 0;
+    for (int k = 0; k < n; k++) {
+        rb.h_off[k] = c;
+        foff[k] = f;
+        for (int h = cut_off[idx[k]]; h < cut_off[idx[k] + 1]; h++, c++) {
+            rb.h_cuts[c].type = cuts[h].type; rb.h_cuts[c].var_index = cuts[h].var_index; rb.h_cuts[c].value = cuts[h].value;
+        }
+        for (int h = fix_off[idx[k]]; h < fix_off[idx[k] + 1]; h++) fx[f++] = fixes[h];
+    }
+    rb.h_off[n] = c;
+    foff[n] = f;
+    nb.cuts = rb.dv_cuts; nb.cut_off = rb.dv_off;
+    if (n <= NODE_INLINE_OFF) {
+        nb.n_inline = n;
+        for (int k = 0; k <= n; k++) nb.cut_off_inline[k] = rb.h_off[k];
+    }
+    // one device block per chunk: fixing offsets, fixings, final columns, final labels
+    const size_t b_fx = (sizeof(int) * (size_t)(n + 1) + 15) & ~(size_t)15;
+    const size_t b_rhs = b_fx + ((sizeof(EditDev) * (size_t)totf + 15) & ~(size_t)15);
+    const size_t b_vrow = b_rhs + sizeof(double) * (size_t)n * nb.Hcap;
+    rc = batch_scratch(t, b_vrow + sizeof(int) * (size_t)n * nb.Hcap);
+    if (rc) return rc;
+    char *base = (char *)t->d_scratch;
+    cudaStream_t s = t->ctx->stream;
+    CK(cudaMemcpyAsync(base, foff.data(), sizeof(int) * (size_t)(n + 1), cudaMemcpyHostToDevice, s));
+    if (totf > 0) CK(cudaMemcpyAsync(base + b_fx, fx.data(), sizeof(EditDev) * (size_t)totf, cudaMemcpyHostToDevice, s));
+    nb.edit_off = (const int *)base;
+    nb.edits = (const EditDev *)(base + b_fx);
+    nb.out_rhs = (double *)(base + b_rhs); nb.out_vrow = (int *)(base + b_vrow);
+    std::vector<double> rhs((size_t)n * nb.Hcap);
+    std::vector<int32_t> vrow((size_t)n * nb.Hcap);
+    rc = batch_launch<NODE_POOL>(t, nb, n, smem, rhs.data(), vrow.data());
+    if (rc) return rc;
+    bool need_full = false;
+    for (int k = 0; k < n; k++) need_full |= check_cycles && !rb.h_out[k].r.overflow && rb.h_out[k].r.log_n > NODE_LOG_HEAD;
+    rc = batch_fetch_logs(t, n, need_full);
+    if (rc) return rc;
+    for (int k = 0; k < n; k++) {
+        const NodeResult &r = rb.h_out[k].r;
+        const int i = idx[k];
+        const bool again =
+            r.overflow || (check_cycles && first_cycle(batch_log(t, k), std::min(r.log_n, t->node_log_cap)) >= 0);
+        if (again) { redo.push_back(i); continue; }
+        const int st = r.status == ST_OPTIMAL ? POOL_OPTIMAL : r.status == ST_UNBOUNDED ? POOL_UNBOUNDED : POOL_INFEASIBLE;
+        o.set(i, st, r.eval_raw, t->precision, r.is_integral, r.branch_var, r.branch_value, r.p1 + r.p2);
+        if (o.is_integral[i]) {
+            const int Hn = H0 + cut_off[i + 1] - cut_off[i];
+            memcpy(o.rhs + (size_t)i * o.row_stride, rhs.data() + (size_t)k * nb.Hcap, sizeof(double) * (size_t)Hn);
+            memcpy(o.vrow + (size_t)i * o.row_stride, vrow.data() + (size_t)k * nb.Hcap, sizeof(int32_t) * (size_t)Hn);
+        }
+    }
+    return JSLP_OK;
+}
+
+extern "C" int jslp_pool_batch(jslp_tab *t, const jslp_fix *fixes, const int32_t *fix_offsets, const jslp_cut *cuts,
+                               const int32_t *cut_offsets, int n_nodes, int check_cycles, int row_stride,
+                               int32_t *status, double *evaluation, int32_t *is_integral, int32_t *branch_var,
+                               double *branch_value, int32_t *pivots, double *rhs, int32_t *vrow) {
+    if (!t) return fail(JSLP_E_INVALID, "tab is NULL");
+    if (n_nodes < 0 || (n_nodes > 0 && (!fix_offsets || !cut_offsets || !status || !evaluation || !is_integral ||
+                                        !branch_var || !branch_value || !pivots || !rhs || !vrow)))
+        return fail(JSLP_E_INVALID, "pool_batch: bad offsets / output arguments");
+    if (!t->saved.valid) return fail(JSLP_E_INVALID, "pool_batch needs a snapshot (jslp_save)");
+    if (t->nOpt > 0) return fail(JSLP_E_UNSUPPORTED, "pool_batch: optional objectives are not supported");
+    if (n_nodes == 0) return JSLP_OK;
+    if (fix_offsets[0] != 0 || cut_offsets[0] != 0) return fail(JSLP_E_INVALID, "pool_batch: offsets[0] must be 0");
+    const int W = t->W, H0 = t->saved.H;
+    for (int i = 0; i < n_nodes; i++) {
+        if (fix_offsets[i + 1] < fix_offsets[i] || cut_offsets[i + 1] < cut_offsets[i])
+            return fail(JSLP_E_INVALID, "pool_batch: offsets must not decrease");
+        if (H0 + cut_offsets[i + 1] - cut_offsets[i] > row_stride)
+            return fail(JSLP_E_INVALID, "pool_batch: row_stride is below a region's height (rows plus cuts)");
+    }
+    const int n_fixes = fix_offsets[n_nodes], n_cuts = cut_offsets[n_nodes];
+    if ((n_fixes > 0 && !fixes) || (n_cuts > 0 && !cuts)) return fail(JSLP_E_INVALID, "pool_batch: fixes / cuts is NULL");
+    std::vector<EditDev> fx((size_t)n_fixes);
+    for (int k = 0; k < n_fixes; k++) {
+        if (fixes[k].column < 1 || fixes[k].column >= W) return fail(JSLP_E_INVALID, "pool_batch: fixed column out of range");
+        fx[k] = EditDev{EDIT_FIX_COL, fixes[k].column, fixes[k].value};
+    }
+    for (int k = 0; k < n_cuts; k++)
+        if ((cuts[k].type != 0 && cuts[k].type != 1) || cuts[k].var_index < 0 || cuts[k].var_index >= t->saved.nVars)
+            return fail(JSLP_E_INVALID, "pool_batch: cut type must be 0 (min) or 1 (max), on a label of the snapshot");
+    CK(cudaSetDevice(t->ctx->device));
+    PoolOut o{status, is_integral, branch_var, pivots, evaluation, branch_value, rhs, vrow, row_stride};
+    const CallerState caller(t);
+    std::vector<int> res, redo;
+    int maxc = 0;
+    for (int i = 0; i < n_nodes; i++) {
+        const int nc = cut_offsets[i + 1] - cut_offsets[i];
+        if (batch_resident(t, H0 + nc)) { res.push_back(i); maxc = std::max(maxc, nc); }
+        else redo.push_back(i);
+    }
+    int rc = JSLP_OK;
+    const int chunk = batch_chunk(H0 + maxc);
+    for (size_t k0 = 0; k0 < res.size() && rc == JSLP_OK; k0 += chunk)
+        rc = pool_resident(t, fx, fix_offsets, cuts, cut_offsets, res.data() + k0,
+                           (int)std::min<size_t>(chunk, res.size() - k0), check_cycles, o, redo);
+    for (size_t k = 0; k < redo.size() && rc == JSLP_OK; k++) {
+        const int i = redo[k];
+        const std::vector<EditDev> mine(fx.begin() + fix_offsets[i], fx.begin() + fix_offsets[i + 1]);
+        rc = pool_hbm(t, mine, cuts + cut_offsets[i], cut_offsets[i + 1] - cut_offsets[i], check_cycles, i, o);
+    }
+    const int rc2 = jslp_restore(t);
+    if (rc == JSLP_OK) rc = rc2;
+    CK(cudaStreamSynchronize(t->ctx->stream));
+    caller.restore(t);
+    return rc;
+}

@@ -9,6 +9,7 @@ from .frontier import Frontier as _frontier
 from .lexicographic import Lexicographic as _lexicographic
 from .model import Model, object_keys
 from .polyopt import Polyopt
+from .pool import Pool as _pool
 from .repair import Repair as _repair
 
 
@@ -78,6 +79,12 @@ class Solver:
         return _repair(self, model, weights, objective=objective, gap=gap, absolute_gap=absolute_gap,
                        precision=precision, validate=validate)
 
+    def Pool(self, model: dict, k=10, gap=0.0, absolute_gap=0.0, precision: Optional[float] = None,
+             validate: bool = False, max_nodes=100000, width=None) -> dict:
+        """The k best distinct integer assignments of a MIP, best first, each with its continuous completion, up to an
+        allowance of the optimum (pool.py, DESIGN.md section 2m).  `width` tunes the speculation only."""
+        return _pool(self, model, k, gap, absolute_gap, precision, validate, max_nodes, width)
+
     def _instance(self, model: Any, precision: Optional[float]) -> Model:
         if isinstance(model, dict):
             options = model.get("options") or {}
@@ -141,3 +148,8 @@ def Repair(model: dict, weights=None, *, objective: bool = True, gap=0.0, absolu
            precision: Optional[float] = None, validate: bool = False) -> dict:
     return solver.Repair(model, weights, objective=objective, gap=gap, absolute_gap=absolute_gap,
                          precision=precision, validate=validate)
+
+
+def Pool(model: dict, k=10, gap=0.0, absolute_gap=0.0, precision: Optional[float] = None, validate: bool = False,
+         max_nodes=100000, width=None) -> dict:
+    return solver.Pool(model, k, gap, absolute_gap, precision, validate, max_nodes, width)

@@ -832,6 +832,38 @@ class GpuTableau:
         self._refresh_dims()
         return {"status": status, "eval_raw": eval_raw, "pivots": pivots, "rhs": rhs, "vrow": vrow}
 
+    def pool_batch(self, regions, check_cycles: Optional[bool] = None) -> dict:
+        """jslp_pool_batch: the region LPs of a solution-pool search (DESIGN.md section 2m).  regions = [(fixings,
+        cuts), ...] with fixings [(column, value), ...] applied in order to the saved snapshot and cuts [(type, varIndex,
+        value), ...] appended as addCutConstraints appends them, then simplex() (the model's cycle check unless
+        check_cycles is given).  Returns the per-region status (0 optimal, 1 infeasible, 2 unbounded, 3 cycled),
+        evaluation, is_integral, branch_var / branch_value, pivots, and rhs / vrow (n x row_stride, written for
+        integral regions: the final column 0 and row labels, height + len(cuts) entries).  Leaves the tableau equal to
+        its snapshot."""
+        n = len(regions)
+        fix_off, cut_off = np.zeros(n + 1, dtype=np.int32), np.zeros(n + 1, dtype=np.int32)
+        for i, (fx, cs) in enumerate(regions):
+            fix_off[i + 1], cut_off[i + 1] = fix_off[i] + len(fx), cut_off[i] + len(cs)
+        fixes = (_lib.Fix * max(1, int(fix_off[-1])))()
+        k = 0
+        for fx, _ in regions:
+            for col, value in fx:
+                fixes[k].column, fixes[k].value = int(col), float(value)
+                k += 1
+        cuts = self._cut_array([c for _, cs in regions for c in cs])
+        stride = self.height + max((len(cs) for _, cs in regions), default=0)
+        status, integral, bvar, pivots = (np.empty(n, dtype=np.int32) for _ in range(4))
+        evaluation, bval = np.empty(n, dtype=np.float64), np.empty(n, dtype=np.float64)
+        rhs, vrow = np.zeros((n, stride), dtype=np.float64), np.zeros((n, stride), dtype=np.int32)
+        cc = self._check_cycles() if check_cycles is None else int(bool(check_cycles))
+        _lib.check(self.context.lib.jslp_pool_batch(
+            self._h(), fixes, fix_off.ctypes.data, cuts, cut_off.ctypes.data, n, cc, stride, status.ctypes.data,
+            evaluation.ctypes.data, integral.ctypes.data, bvar.ctypes.data, bval.ctypes.data, pivots.ctypes.data,
+            rhs.ctypes.data, vrow.ctypes.data))
+        self._refresh_dims()
+        return {"status": status, "evaluation": evaluation, "is_integral": integral, "branch_var": bvar,
+                "branch_value": bval, "pivots": pivots, "rhs": rhs, "vrow": vrow}
+
     def column(self, col: int) -> np.ndarray:
         """jslp_column: column `col` of the current tableau (height doubles), without downloading the rest."""
         out = np.empty(self.height, dtype=np.float64)
