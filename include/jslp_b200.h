@@ -383,6 +383,29 @@ int jslp_pool_batch(jslp_tab *tab, const jslp_fix *fixes, const int32_t *fix_off
                     double *evaluation, int32_t *is_integral, int32_t *branch_var, double *branch_value,
                     int32_t *pivots, double *rhs, int32_t *vrow);
 
+/* The node LPs of the feasibility searches behind a MIP conflict, DESIGN.md section 2n.  Node i is cost row 0 plus the
+ * rows r >= 1 of the saved snapshot with keep[i * H + r] != 0 (H = the snapshot's height; row 0 is always kept), in
+ * their original order, followed by the cut rows cuts[cut_offsets[i] .. cut_offsets[i+1]) appended as jslp_add_cuts
+ * appends them (labels from the snapshot's lastElementIndex), then the reference's phase 1 with the cycle check on,
+ * then the isIntegral / getMostFractionalVar scan over the integer variables whose position p in the model's integer
+ * list has int_keep[i * n_int + p] != 0 (n_int = the number of integer variables; int_keep may be NULL when it is 0).
+ * Nodes whose rows fit shared memory run one CTA each in one launch; the others, and any node that hits the in-kernel
+ * pivot or log cap, run one after another on the single-tableau path.  Per node:
+ *   status         0 feasible (phase 1 ended with no leaving row), 1 infeasible, 2 cycled (stopped before the pivot
+ *                  that completes the repeat)
+ *   is_integral    1 when feasible and every basic integer variable of the mask is integral
+ *   branch_var / branch_value   the most fractional integer variable of the mask when feasible and not integral
+ *                  (lowest position on ties), else -1 / 0
+ *   pivots         phase-1 pivots
+ *   rhs, vrow      row_stride entries each at i * row_stride; unless the node cycled, the first 1 + kept rows + cuts
+ *                  hold the final column 0 and row labels, otherwise they are not written
+ * row_stride must be at least every node's height (1 + kept rows + cuts).  Needs a snapshot (jslp_save); on return the
+ * tableau equals it, and the scalar Tableau state and executed-pivot log are as they were.  No optional objectives
+ * (JSLP_E_UNSUPPORTED). */
+int jslp_conflict_batch(jslp_tab *tab, const uint8_t *keep, const uint8_t *int_keep, const jslp_cut *cuts,
+                        const int32_t *cut_offsets, int n_nodes, int row_stride, int32_t *status, int32_t *is_integral,
+                        int32_t *branch_var, double *branch_value, int32_t *pivots, double *rhs, int32_t *vrow);
+
 /* Column `col` (0..W-1) of the current tableau, H doubles, into out: one strided device-to-host copy, so a single
  * column of a large tableau is read without downloading the whole of it. */
 int jslp_column(jslp_tab *tab, int col, double *out);

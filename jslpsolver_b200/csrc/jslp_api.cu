@@ -1382,3 +1382,4 @@ extern "C" int jslp_pivot_log(jslp_tab *t, int32_t *entries, int cap, int *n) {
 #include "jslp_elastic.cuh"
 #include "jslp_cone.cuh"
 #include "jslp_pool.cuh"
+#include "jslp_conflict.cuh"

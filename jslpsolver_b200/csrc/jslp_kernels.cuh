@@ -979,8 +979,10 @@ __global__ void __launch_bounds__(256) k_mir_cuts(const TabDev *Tp, int H0, int 
     if (tid == 0) *n_added = n;
 }
 
-// isIntegral + getMostFractionalVar (mip-utils.ts:43-61,100-126) over the RHS column.
-__device__ __forceinline__ void cta_mip_scan(const TabDev &T, MipOut *out, RedSmem &red) {
+// isIntegral + getMostFractionalVar (mip-utils.ts:43-61,100-126) over the RHS column.  MASKED (DESIGN.md 2n): only
+// the integer variables whose position p in model.integerVariables has bit p set in imask take part.
+template <bool MASKED = false>
+__device__ __forceinline__ void cta_mip_scan(const TabDev &T, MipOut *out, RedSmem &red, const uint32_t *imask = nullptr) {
     const VI init = {0.0, INT_MAX};
     VI best = init;  // (fraction, position in model.integerVariables)
     int nonint = 0;
@@ -989,6 +991,7 @@ __device__ __forceinline__ void cta_mip_scan(const TabDev &T, MipOut *out, RedSm
         if (v < 0 || v >= T.n_index) continue;
         const int p = T.intpos[v];
         if (p < 0) continue;
+        if (MASKED && !((imask[p >> 5] >> (p & 31)) & 1u)) continue;
         const double x = T.M[(size_t)r * T.stride];
         const double fr = fabs(x - js_round(x));
         if (fr > T.prec) nonint = 1;

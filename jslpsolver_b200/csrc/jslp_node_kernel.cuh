@@ -46,6 +46,8 @@ enum NodeMode : int {
     NODE_SCENARIO = 2,  // one list of right-hand-side / cost edits of the root per CTA (jslp_scenario_batch)
     NODE_COLUMNS = 3,   // one column subset of the root per CTA, the others zeroed (jslp_column_batch)
     NODE_POOL = 4,      // one region of a solution-pool search per CTA: fixed columns, then cut rows (jslp_pool_batch)
+    NODE_CONFLICT = 5,  // one node of a conflict search per CTA: a row subset, then cut rows, phase 1 only, and the
+                        // integrality scan over an integer mask (jslp_conflict_batch)
 };
 
 // One resolved scenario edit (DESIGN.md 2e): where updateRightHandSide / updateCost (dynamic-modification.ts:78-160)
@@ -93,6 +95,13 @@ struct NodeBatchDev {
     int *out_vrow;
     int n_inline;         // > 0: cut_off_inline holds the n_inline + 1 offsets (saves a PCIe round trip)
     int cut_off_inline[NODE_INLINE_OFF + 1];
+    // Conflict launches (NODE_CONFLICT, jslp_conflict_batch) keep the root rows of keep as NODE_SUBSET does, append the
+    // node's cut rows after them and stop where phase 1 ends; Hcap counts the kept rows plus the cuts of the largest
+    // node.  The integrality scan reads only the integer positions p whose bit is set in int_keep[n * int_words ...]
+    // (device memory), and column 0 and the row labels go to out_rhs / out_vrow + n * Hcap.  Not read by the other
+    // modes.
+    const uint32_t *int_keep;
+    int int_words;
 };
 
 constexpr int NODE_THREADS = 256;
@@ -155,12 +164,15 @@ struct NodePart {    // per-warp partial results of a scan
 // unrestricted lookup and the pivot log read as on the whole tableau.  NODE_SCENARIO: every root row, then the CTA's
 // edit list applied to column 0 and row 0 (DESIGN.md 2e) in place of cut rows.  NODE_COLUMNS: every root row, with the
 // columns cleared in the CTA's mask set to +0 in every row, row 0 included (DESIGN.md 2l).  NODE_POOL: every root row,
-// the CTA's fixings applied by the scenario edit loop, then its cut rows (DESIGN.md 2m).  A template parameter, so
-// that the node path carries none of the subset, scenario, column or pool code.
+// the CTA's fixings applied by the scenario edit loop, then its cut rows (DESIGN.md 2m).  NODE_CONFLICT: SUBSET's row
+// subset followed by the CTA's cut rows, phase 1 only, and the integrality scan over the CTA's integer mask (DESIGN.md
+// 2n).  A template parameter, so that the node path carries none of the subset, scenario, column, pool or conflict
+// code.
 template <int MODE>
 __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, const __grid_constant__ NodeBatchDev nb) {
     constexpr bool SUBSET = MODE == NODE_SUBSET, SCENARIO = MODE == NODE_SCENARIO, COLUMNS = MODE == NODE_COLUMNS;
-    constexpr bool POOL = MODE == NODE_POOL;
+    constexpr bool POOL = MODE == NODE_POOL, CONFLICT = MODE == NODE_CONFLICT;
+    constexpr bool KEEP = SUBSET || CONFLICT;  // a row subset of the root, compacted in row order
     extern __shared__ __align__(16) unsigned char smraw[];
     __shared__ TabDev T;
     __shared__ SelSmem sel;
@@ -186,7 +198,7 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
     double *frow = Ms + (size_t)(nb.Hcap + 1) * Ws;
     double *rhs = frow + Ws;                         // Hcap entries: pivot-column staging, final RHS column
     CutDev *cutS = reinterpret_cast<CutDev *>(rhs + nb.Hcap + (nb.Hcap & 1));
-    int *vrow = reinterpret_cast<int *>(cutS + (nb.Hcap - H0));
+    int *vrow = reinterpret_cast<int *>(cutS + (CONFLICT ? nb.Hcap : nb.Hcap - H0));
     int *slot = vrow + nb.Hcap;
     if (tid == 0) {
         T = *Tp;
@@ -197,7 +209,7 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
     }
     __syncthreads();
     int H0k = H0;  // rows restored from the root
-    if constexpr (SUBSET) {
+    if constexpr (KEEP) {
         // compacted position of every kept row: slot[d] = the root row that becomes row d (slot is reset below,
         // once the copies that read it have been issued)
         if (warp == 0) {
@@ -219,7 +231,7 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
     if (tid == 0) mbar_expect_tx(&s_bar, (uint32_t)(H0k * Ws * sizeof(double)));
     __syncthreads();
     for (int r = tid; r < H0k; r += NT) {
-        const int src = SUBSET ? slot[r] : r;
+        const int src = KEEP ? slot[r] : r;
         tma_bulk_g2s(Ms + (size_t)r * Ws, nb.rootM + (size_t)src * nb.root_stride, (uint32_t)(Ws * sizeof(double)), &s_bar);
     }
     // the cut list may live in mapped host memory: one PCIe round trip, overlapped with the restore
@@ -231,15 +243,15 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
     const double prec = T.prec;
     int *vcol = T.vcol;
     for (int h = tid; !SCENARIO && !COLUMNS && h < nc; h += NT) cutS[h] = nb.cuts[c0 + h];
-    for (int r = tid; r < H0k; r += NT) vrow[r] = __ldg(nb.root_vrow + (SUBSET ? slot[r] : r));
+    for (int r = tid; r < H0k; r += NT) vrow[r] = __ldg(nb.root_vrow + (KEEP ? slot[r] : r));
     for (int c = tid; c < W; c += NT) vcol[c] = __ldg(nb.root_vcol + c);
-    if (!SUBSET)
+    if (!KEEP)
         for (int r = tid; r < nb.Hcap; r += NT) slot[r] = r;
     const int Hn = (SCENARIO || COLUMNS) ? H0k : H0k + nc;
     if (tid == 0) tl0 = globaltimer_ns() - t_start;
     mbar_wait(&s_bar, 0);
     __syncthreads();
-    if (SUBSET)  // nobody reads slot until the barrier after the cut rows
+    if (KEEP)  // nobody reads slot until the barrier after the cut rows
         for (int r = tid; r < nb.Hcap; r += NT) slot[r] = r;
     if (tid == 0) tl1 = globaltimer_ns() - t_start;
     if constexpr (SCENARIO || POOL) {
@@ -339,7 +351,7 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
                 }
                 b = warp_reduce_vi<true>(b);
                 if (b.i == INT_MAX) {  // feasible (simplex.ts:51-54)
-                    if (SUBSET && nb.phase1_only) { status = ST_P1_DONE; go = 0; }
+                    if (CONFLICT || (SUBSET && nb.phase1_only)) { status = ST_P1_DONE; go = 0; }
                     else phase = 2;
                 } else {
                     rstar = b.i;
@@ -515,7 +527,7 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
     // isIntegral / most fractional variable over the final RHS column
     for (int r = tid; r < Hn; r += NT) rhs[r] = Ms[(size_t)slot[r] * Ws];
     __syncthreads();
-    if constexpr (SCENARIO || COLUMNS || POOL)
+    if constexpr (SCENARIO || COLUMNS || POOL || CONFLICT)
         for (int r = tid; r < Hn; r += NT) {
             nb.out_rhs[(size_t)node * nb.Hcap + r] = rhs[r];
             nb.out_vrow[(size_t)node * nb.Hcap + r] = vrow[r];
@@ -523,7 +535,7 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
     if (T.intpos != nullptr) {
         if (tid == 0) { T.M = rhs; T.stride = 1; T.vrow = vrow; T.H = Hn; }
         __syncthreads();
-        cta_mip_scan(T, &mip, sel.red);
+        cta_mip_scan<CONFLICT>(T, &mip, sel.red, CONFLICT ? nb.int_keep + (size_t)node * nb.int_words : nullptr);
     } else if (tid == 0) { mip.is_integral = 1; mip.var_index = -1; mip.value = 0.0; }
     __syncthreads();
     if (tid == 0) tl4 = globaltimer_ns() - t_start;

@@ -278,6 +278,42 @@ def planted_unbounded_model(n_vars: int, n_cons: int, n_solo: int, n_pairs: int,
             "opType": "max", "constraints": constraints, "variables": variables}
 
 
+def planted_integer_conflict_model(n_vars: int, n_cons: int, k: int, seed: int = 12345) -> dict:
+    """max c.x over a dense packing MIP with one planted parity equality, without an integer plan by construction.
+    n_vars counts every variable `x{j}` (all integer), n_cons every row; the equality `parity` is two of them (its
+    `min` row, then its `max` row) at a seeded position among the packing rows.  Packing rows are a_i.x <= b_i with
+    a_ij ~ U{1..20} and b_i ~ U{100..500}; costs are U{1..50}.  The parity row is sum_j 2 x_j = 2m + 1, m ~ U{0..1},
+    over k planted columns at seeded positions: an even sum is never odd, so no integer plan exists.  Dropping the
+    `max` half leaves x_j = m + 1 at one planted column, dropping the `min` half leaves x = 0, and dropping the
+    integrality of one planted column leaves x_j = m + 1/2 there; each satisfies every packing row (20 * 2 <= 100).
+    So the only conflict is both parity rows plus the integrality of the k planted columns."""
+    rng = np.random.default_rng(seed)
+    r_pack = n_cons - 2
+    if k < 1 or k > n_vars or r_pack < 0:
+        raise ValueError("planted_integer_conflict_model: needs 1 <= k <= n_vars and n_cons >= 2")
+    m = int(rng.integers(0, 2))
+    planted = set(int(j) for j in rng.choice(n_vars, size=k, replace=False))
+    at = int(rng.integers(0, r_pack + 1))
+    A = rng.integers(1, 21, size=(r_pack, n_vars)).astype(np.float64)
+    b = rng.integers(100, 501, size=r_pack).astype(np.float64)
+    constraints = {}
+    for i in range(r_pack + 1):
+        if i == at:
+            constraints["parity"] = {"equal": float(2 * m + 1)}
+        if i < r_pack:
+            constraints[f"resource{i}"] = {"max": float(b[i])}
+    variables = {}
+    for j in range(n_vars):
+        v = {"profit": float(rng.integers(1, 51))}
+        for i in range(r_pack):
+            v[f"resource{i}"] = float(A[i, j])
+        if j in planted:
+            v["parity"] = 2.0
+        variables[f"x{j}"] = v
+    return {"name": f"PlantedIntegerConflict_{n_vars}x{n_cons}_{k}_seed{seed}", "optimize": "profit", "opType": "max",
+            "constraints": constraints, "variables": variables, "ints": {f"x{j}": 1 for j in range(n_vars)}}
+
+
 def knapsack_mip_model(n_items: int, n_cons: int, seed: int = 12345, tolerance: float = 0.0) -> dict:
     """Multi-dimensional 0/1 knapsack (SURVEY.md 8d config 5): a_ij ~ U{1..50} dense,
     b_i = floor(0.5 * sum_j a_ij), c_j ~ U{1..50}; every binary adds an `x <= 1` row

@@ -5,6 +5,7 @@ from __future__ import annotations
 from typing import Any, Optional
 
 from . import validation
+from .conflict import Conflict as _conflict
 from .frontier import Frontier as _frontier
 from .lexicographic import Lexicographic as _lexicographic
 from .model import Model, object_keys
@@ -85,6 +86,12 @@ class Solver:
         allowance of the optimum (pool.py, DESIGN.md section 2m).  `width` tunes the speculation only."""
         return _pool(self, model, k, gap, absolute_gap, precision, validate, max_nodes, width)
 
+    def Conflict(self, model: dict, max_nodes=10000, width=None, depth=None, precision: Optional[float] = None,
+                 validate: bool = False) -> dict:
+        """An irreducible set of rows and integrality restrictions of a MIP that has no integer plan, each member with
+        the plan that breaks only it (conflict.py, DESIGN.md section 2n).  `width` / `depth` tune the batching only."""
+        return _conflict(self, model, max_nodes, width, depth, precision, validate)
+
     def _instance(self, model: Any, precision: Optional[float]) -> Model:
         if isinstance(model, dict):
             options = model.get("options") or {}
@@ -153,3 +160,8 @@ def Repair(model: dict, weights=None, *, objective: bool = True, gap=0.0, absolu
 def Pool(model: dict, k=10, gap=0.0, absolute_gap=0.0, precision: Optional[float] = None, validate: bool = False,
          max_nodes=100000, width=None) -> dict:
     return solver.Pool(model, k, gap, absolute_gap, precision, validate, max_nodes, width)
+
+
+def Conflict(model: dict, max_nodes=10000, width=None, depth=None, precision: Optional[float] = None,
+             validate: bool = False) -> dict:
+    return solver.Conflict(model, max_nodes, width, depth, precision, validate)

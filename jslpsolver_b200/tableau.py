@@ -864,6 +864,33 @@ class GpuTableau:
         return {"status": status, "evaluation": evaluation, "is_integral": integral, "branch_var": bvar,
                 "branch_value": bval, "pivots": pivots, "rhs": rhs, "vrow": vrow}
 
+    def conflict_batch(self, keep, int_keep, cuts) -> dict:
+        """jslp_conflict_batch: the node LPs of a MIP conflict search (DESIGN.md section 2n).  keep (n x height,
+        nonzero = keep; row 0 is always kept) selects rows of the saved snapshot, int_keep (n x integer variables, in
+        integerIndices order) the integrality the scan checks, and cuts[i] = [(type, varIndex, value), ...] the cut
+        rows appended after the kept rows; then phase 1 with the cycle check on.  Returns the per-node status (0
+        feasible, 1 infeasible, 2 cycled), is_integral, branch_var / branch_value, pivots, and rhs / vrow (n x
+        row_stride: the final column 0 and row labels, 1 + kept rows + cuts entries, unless the node cycled).  Leaves
+        the tableau equal to its snapshot."""
+        keep = np.ascontiguousarray(keep, dtype=np.uint8)
+        int_keep = np.ascontiguousarray(int_keep, dtype=np.uint8)
+        n = keep.shape[0]
+        cut_off = np.zeros(n + 1, dtype=np.int32)
+        for i, cs in enumerate(cuts):
+            cut_off[i + 1] = cut_off[i] + len(cs)
+        arr = self._cut_array([c for cs in cuts for c in cs])
+        stride = int(keep[:, 1:].astype(bool).sum(axis=1).max(initial=0)) + 1 + max((len(cs) for cs in cuts), default=0)
+        status, integral, bvar, pivots = (np.empty(n, dtype=np.int32) for _ in range(4))
+        bval = np.empty(n, dtype=np.float64)
+        rhs, vrow = np.zeros((n, stride), dtype=np.float64), np.zeros((n, stride), dtype=np.int32)
+        _lib.check(self.context.lib.jslp_conflict_batch(
+            self._h(), keep.ctypes.data, int_keep.ctypes.data if int_keep.size else None, arr, cut_off.ctypes.data, n,
+            stride, status.ctypes.data, integral.ctypes.data, bvar.ctypes.data, bval.ctypes.data, pivots.ctypes.data,
+            rhs.ctypes.data, vrow.ctypes.data))
+        self._refresh_dims()
+        return {"status": status, "is_integral": integral, "branch_var": bvar, "branch_value": bval,
+                "pivots": pivots, "rhs": rhs, "vrow": vrow}
+
     def column(self, col: int) -> np.ndarray:
         """jslp_column: column `col` of the current tableau (height doubles), without downloading the rest."""
         out = np.empty(self.height, dtype=np.float64)
