@@ -97,8 +97,8 @@ static int column_resident(jslp_tab *t, const uint32_t *bits, int words, int s0,
     size_t smem = 0;
     int rc = batch_fill(t, t->saved.M, t->saved.vrow, t->saved.vcol, H0, t->saved.lastElementIndex, n, nb, &smem);
     if (rc) return rc;
-    for (int i = 0; i <= n; i++) rb.h_off[i] = 0;  // no cut rows
-    nb.cuts = rb.dv_cuts; nb.cut_off = rb.dv_off;
+    rc = batch_cuts(t, nullptr, nullptr, nullptr, n, nb);  // no cut rows
+    if (rc) return rc;
     // one device block per chunk: masks, final columns, final labels
     const size_t b_rhs = (sizeof(uint32_t) * (size_t)n * words + 15) & ~(size_t)15;
     const size_t b_vrow = b_rhs + sizeof(double) * (size_t)n * H0;
@@ -109,7 +109,6 @@ static int column_resident(jslp_tab *t, const uint32_t *bits, int words, int s0,
                        t->ctx->stream));
     nb.keep = (const uint32_t *)base; nb.keep_words = words;
     nb.out_rhs = (double *)(base + b_rhs); nb.out_vrow = (int *)(base + b_vrow);
-    if (n <= NODE_INLINE_OFF) nb.n_inline = n;  // cut_off_inline: all zero
     rc = batch_launch<NODE_COLUMNS>(t, nb, n, smem, rhs + (size_t)s0 * H0, vrow + (size_t)s0 * H0);
     if (rc) return rc;
     bool need_full = false;
@@ -139,10 +138,8 @@ extern "C" int jslp_column_batch(jslp_tab *t, const uint8_t *keep_cols, int n_se
     const int W = t->W, H0 = t->saved.H;
     // keep masks, bit-packed over the columns (column 0 always kept)
     const int words = (W + 31) / 32;
-    std::vector<uint32_t> bits((size_t)n_sets * words, 0u);
-    for (int i = 0; i < n_sets; i++)
-        for (int c = 0; c < W; c++)
-            if (c == 0 || keep_cols[(size_t)i * W + c]) bits[(size_t)i * words + (c >> 5)] |= 1u << (c & 31);
+    std::vector<uint32_t> bits = pack_bits(keep_cols, W, nullptr, n_sets, words);
+    for (int i = 0; i < n_sets; i++) bits[(size_t)i * words] |= 1u;
     const CallerState caller(t);
     std::vector<int> redo;
     int rc = JSLP_OK;

@@ -42,12 +42,11 @@ constexpr int NODE_INLINE_OFF = 64;
 // Launch modes of k_node_batch (a template parameter: each mode's instantiation carries only its own prologue)
 enum NodeMode : int {
     NODE_BRANCH = 0,    // branch-and-cut nodes and engine 4: every root row, then the node's cuts
-    NODE_SUBSET = 1,    // one row subset of the root per CTA (jslp_feasibility_batch)
     NODE_SCENARIO = 2,  // one list of right-hand-side / cost edits of the root per CTA (jslp_scenario_batch)
     NODE_COLUMNS = 3,   // one column subset of the root per CTA, the others zeroed (jslp_column_batch)
     NODE_POOL = 4,      // one region of a solution-pool search per CTA: fixed columns, then cut rows (jslp_pool_batch)
-    NODE_CONFLICT = 5,  // one node of a conflict search per CTA: a row subset, then cut rows, phase 1 only, and the
-                        // integrality scan over an integer mask (jslp_conflict_batch)
+    NODE_CONFLICT = 5,  // one row subset of the root per CTA, then cut rows, phase 1 only, and the integrality scan
+                        // over an integer mask (jslp_conflict_batch; jslp_feasibility_batch without cuts or mask)
 };
 
 // One resolved scenario edit (DESIGN.md 2e): where updateRightHandSide / updateCost (dynamic-modification.ts:78-160)
@@ -75,13 +74,12 @@ struct NodeBatchDev {
     double *wb_M;          // optional write-back of node 0's final tableau (stride = root_stride)
     int *wb_vrow, *wb_vcol;
     int H0, root_stride, first_index, Hcap, Ws, log_cap, max_pivots;
-    // row-subset launches (NODE_SUBSET, jslp_feasibility_batch): node n keeps the root rows whose bits are set
-    // in keep[n * keep_words ...] (device memory; row 0 is always kept), and with phase1_only the CTA stops with
-    // ST_P1_DONE where phase 1 finds no leaving row.  Column-subset launches (NODE_COLUMNS, jslp_column_batch) read
-    // the same bits as columns: node n writes +0 over every column whose bit is clear, in every row.  Not read by
-    // the other modes.
+    // row-subset launches (NODE_CONFLICT): node n keeps the root rows whose bits are set in keep[n * keep_words ...]
+    // (device memory; row 0 is always kept).  Column-subset launches (NODE_COLUMNS, jslp_column_batch) read the same
+    // bits as columns: node n writes +0 over every column whose bit is clear, in every row.  Not read by the other
+    // modes.
     const uint32_t *keep;
-    int keep_words, phase1_only;
+    int keep_words;
     // scenario launches (NODE_SCENARIO, jslp_scenario_batch): node n applies edits[cut_off[n] .. cut_off[n+1]) (device
     // memory; every right-hand-side edit before every cost edit) to the restored root, solves, and writes its final
     // column 0 and row labels to out_rhs / out_vrow + n * Hcap (NODE_COLUMNS writes them too).  Not read by the other
@@ -95,11 +93,12 @@ struct NodeBatchDev {
     int *out_vrow;
     int n_inline;         // > 0: cut_off_inline holds the n_inline + 1 offsets (saves a PCIe round trip)
     int cut_off_inline[NODE_INLINE_OFF + 1];
-    // Conflict launches (NODE_CONFLICT, jslp_conflict_batch) keep the root rows of keep as NODE_SUBSET does, append the
-    // node's cut rows after them and stop where phase 1 ends; Hcap counts the kept rows plus the cuts of the largest
-    // node.  The integrality scan reads only the integer positions p whose bit is set in int_keep[n * int_words ...]
-    // (device memory), and column 0 and the row labels go to out_rhs / out_vrow + n * Hcap.  Not read by the other
-    // modes.
+    // Row-subset launches (NODE_CONFLICT: jslp_conflict_batch, and jslp_feasibility_batch without cuts, mask or
+    // outputs) append the node's cut rows after its kept rows and stop with ST_P1_DONE where phase 1 finds no leaving
+    // row; Hcap counts the kept rows plus the cuts of the largest node.  With int_keep set, the integrality scan reads
+    // only the integer positions p whose bit is set in int_keep[n * int_words ...] (device memory); with it null there
+    // is no scan.  With out_rhs set, column 0 and the row labels go to out_rhs / out_vrow + n * Hcap.  Not read by the
+    // other modes.
     const uint32_t *int_keep;
     int int_words;
 };
@@ -159,20 +158,18 @@ struct NodePart {    // per-warp partial results of a scan
     int i[8], d[8], n[8];
 };
 
-// MODE = NODE_BRANCH: branch-and-cut nodes and engine 4 (every root row, then the node's cuts).  NODE_SUBSET: one row
-// subset of the root per CTA (NodeBatchDev.keep), compacted in row order; row labels stay the root's, so the
-// unrestricted lookup and the pivot log read as on the whole tableau.  NODE_SCENARIO: every root row, then the CTA's
-// edit list applied to column 0 and row 0 (DESIGN.md 2e) in place of cut rows.  NODE_COLUMNS: every root row, with the
-// columns cleared in the CTA's mask set to +0 in every row, row 0 included (DESIGN.md 2l).  NODE_POOL: every root row,
-// the CTA's fixings applied by the scenario edit loop, then its cut rows (DESIGN.md 2m).  NODE_CONFLICT: SUBSET's row
-// subset followed by the CTA's cut rows, phase 1 only, and the integrality scan over the CTA's integer mask (DESIGN.md
-// 2n).  A template parameter, so that the node path carries none of the subset, scenario, column, pool or conflict
-// code.
+// MODE = NODE_BRANCH: branch-and-cut nodes and engine 4 (every root row, then the node's cuts).  NODE_SCENARIO: every
+// root row, then the CTA's edit list applied to column 0 and row 0 (DESIGN.md 2e) in place of cut rows.  NODE_COLUMNS:
+// every root row, with the columns cleared in the CTA's mask set to +0 in every row, row 0 included (DESIGN.md 2l).
+// NODE_POOL: every root row, the CTA's fixings applied by the scenario edit loop, then its cut rows (DESIGN.md 2m).
+// NODE_CONFLICT: one row subset of the root per CTA (NodeBatchDev.keep), compacted in row order, then the CTA's cut
+// rows, phase 1 only, and the integrality scan over the CTA's integer mask if it has one (DESIGN.md 2c, 2n); row
+// labels stay the root's, so the unrestricted lookup and the pivot log read as on the whole tableau.  A template
+// parameter, so that the node path carries none of the scenario, column, pool or row-subset code.
 template <int MODE>
 __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, const __grid_constant__ NodeBatchDev nb) {
-    constexpr bool SUBSET = MODE == NODE_SUBSET, SCENARIO = MODE == NODE_SCENARIO, COLUMNS = MODE == NODE_COLUMNS;
+    constexpr bool SCENARIO = MODE == NODE_SCENARIO, COLUMNS = MODE == NODE_COLUMNS;
     constexpr bool POOL = MODE == NODE_POOL, CONFLICT = MODE == NODE_CONFLICT;
-    constexpr bool KEEP = SUBSET || CONFLICT;  // a row subset of the root, compacted in row order
     extern __shared__ __align__(16) unsigned char smraw[];
     __shared__ TabDev T;
     __shared__ SelSmem sel;
@@ -209,7 +206,7 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
     }
     __syncthreads();
     int H0k = H0;  // rows restored from the root
-    if constexpr (KEEP) {
+    if constexpr (CONFLICT) {
         // compacted position of every kept row: slot[d] = the root row that becomes row d (slot is reset below,
         // once the copies that read it have been issued)
         if (warp == 0) {
@@ -231,7 +228,7 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
     if (tid == 0) mbar_expect_tx(&s_bar, (uint32_t)(H0k * Ws * sizeof(double)));
     __syncthreads();
     for (int r = tid; r < H0k; r += NT) {
-        const int src = KEEP ? slot[r] : r;
+        const int src = CONFLICT ? slot[r] : r;
         tma_bulk_g2s(Ms + (size_t)r * Ws, nb.rootM + (size_t)src * nb.root_stride, (uint32_t)(Ws * sizeof(double)), &s_bar);
     }
     // the cut list may live in mapped host memory: one PCIe round trip, overlapped with the restore
@@ -243,15 +240,15 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
     const double prec = T.prec;
     int *vcol = T.vcol;
     for (int h = tid; !SCENARIO && !COLUMNS && h < nc; h += NT) cutS[h] = nb.cuts[c0 + h];
-    for (int r = tid; r < H0k; r += NT) vrow[r] = __ldg(nb.root_vrow + (KEEP ? slot[r] : r));
+    for (int r = tid; r < H0k; r += NT) vrow[r] = __ldg(nb.root_vrow + (CONFLICT ? slot[r] : r));
     for (int c = tid; c < W; c += NT) vcol[c] = __ldg(nb.root_vcol + c);
-    if (!KEEP)
+    if (!CONFLICT)
         for (int r = tid; r < nb.Hcap; r += NT) slot[r] = r;
     const int Hn = (SCENARIO || COLUMNS) ? H0k : H0k + nc;
     if (tid == 0) tl0 = globaltimer_ns() - t_start;
     mbar_wait(&s_bar, 0);
     __syncthreads();
-    if (KEEP)  // nobody reads slot until the barrier after the cut rows
+    if (CONFLICT)  // nobody reads slot until the barrier after the cut rows
         for (int r = tid; r < nb.Hcap; r += NT) slot[r] = r;
     if (tid == 0) tl1 = globaltimer_ns() - t_start;
     if constexpr (SCENARIO || POOL) {
@@ -351,7 +348,7 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
                 }
                 b = warp_reduce_vi<true>(b);
                 if (b.i == INT_MAX) {  // feasible (simplex.ts:51-54)
-                    if (CONFLICT || (SUBSET && nb.phase1_only)) { status = ST_P1_DONE; go = 0; }
+                    if (CONFLICT) { status = ST_P1_DONE; go = 0; }
                     else phase = 2;
                 } else {
                     rstar = b.i;
@@ -528,11 +525,13 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
     for (int r = tid; r < Hn; r += NT) rhs[r] = Ms[(size_t)slot[r] * Ws];
     __syncthreads();
     if constexpr (SCENARIO || COLUMNS || POOL || CONFLICT)
-        for (int r = tid; r < Hn; r += NT) {
-            nb.out_rhs[(size_t)node * nb.Hcap + r] = rhs[r];
-            nb.out_vrow[(size_t)node * nb.Hcap + r] = vrow[r];
-        }
-    if (T.intpos != nullptr) {
+        if (!CONFLICT || nb.out_rhs != nullptr)  // a row-subset launch writes them only when asked
+            for (int r = tid; r < Hn; r += NT) {
+                nb.out_rhs[(size_t)node * nb.Hcap + r] = rhs[r];
+                nb.out_vrow[(size_t)node * nb.Hcap + r] = vrow[r];
+            }
+    // a row-subset launch without an integer mask has no scan: integral, as a tableau without integer variables
+    if (T.intpos != nullptr && (!CONFLICT || nb.int_keep != nullptr)) {
         if (tid == 0) { T.M = rhs; T.stride = 1; T.vrow = vrow; T.H = Hn; }
         __syncthreads();
         cta_mip_scan<CONFLICT>(T, &mip, sel.red, CONFLICT ? nb.int_keep + (size_t)node * nb.int_words : nullptr);

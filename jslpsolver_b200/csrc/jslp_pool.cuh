@@ -90,40 +90,27 @@ static int pool_resident(jslp_tab *t, const std::vector<EditDev> &fixes, const i
                          std::vector<int> &redo) {
     ResidentBufs &rb = t->rbufs;
     const int H0 = t->saved.H;
-    int maxc = 0, totc = 0, totf = 0;
+    int maxc = 0, totf = 0;
     for (int k = 0; k < n; k++) {
-        const int nc = cut_off[idx[k] + 1] - cut_off[idx[k]];
-        maxc = std::max(maxc, nc);
-        totc += nc;
+        maxc = std::max(maxc, cut_off[idx[k] + 1] - cut_off[idx[k]]);
         totf += fix_off[idx[k] + 1] - fix_off[idx[k]];
     }
-    int rc = rb.ensure(n, totc, t->node_log_cap);
-    if (rc) return rc;
     NodeBatchDev nb;
     size_t smem = 0;
-    rc = batch_fill(t, t->saved.M, t->saved.vrow, t->saved.vcol, H0, t->saved.lastElementIndex, n, nb, &smem);
+    int rc = batch_fill(t, t->saved.M, t->saved.vrow, t->saved.vcol, H0, t->saved.lastElementIndex, n, nb, &smem);
+    if (rc) return rc;
+    rc = batch_cuts(t, cuts, cut_off, idx, n, nb);
     if (rc) return rc;
     nb.Hcap = H0 + maxc;
     smem = node_smem_bytes(nb.Hcap, t->W, nullptr);
-    // cut rows: mapped host memory, as branch-and-cut's node launches read them
     std::vector<int> foff((size_t)n + 1);
     std::vector<EditDev> fx((size_t)std::max(1, totf));
-    int c = 0, f = 0;
+    int f = 0;
     for (int k = 0; k < n; k++) {
-        rb.h_off[k] = c;
         foff[k] = f;
-        for (int h = cut_off[idx[k]]; h < cut_off[idx[k] + 1]; h++, c++) {
-            rb.h_cuts[c].type = cuts[h].type; rb.h_cuts[c].var_index = cuts[h].var_index; rb.h_cuts[c].value = cuts[h].value;
-        }
         for (int h = fix_off[idx[k]]; h < fix_off[idx[k] + 1]; h++) fx[f++] = fixes[h];
     }
-    rb.h_off[n] = c;
     foff[n] = f;
-    nb.cuts = rb.dv_cuts; nb.cut_off = rb.dv_off;
-    if (n <= NODE_INLINE_OFF) {
-        nb.n_inline = n;
-        for (int k = 0; k <= n; k++) nb.cut_off_inline[k] = rb.h_off[k];
-    }
     // one device block per chunk: fixing offsets, fixings, final columns, final labels
     const size_t b_fx = (sizeof(int) * (size_t)(n + 1) + 15) & ~(size_t)15;
     const size_t b_rhs = b_fx + ((sizeof(EditDev) * (size_t)totf + 15) & ~(size_t)15);

@@ -21,10 +21,10 @@ from test_gpu_shape_edges import device, resident_rows, solved
 pytestmark = pytest.mark.gpu
 
 # ------------------------------------------------------------------ the node kernel's geometry, restated
-NODE_THREADS = 256      # jslp_node_kernel.cuh:87 (NODE_THREADS): 8 warps, one partial each in S2 / S3 (:344, :366)
+NODE_THREADS = 256      # jslp_node_kernel.cuh:106 (NODE_THREADS): 8 warps, one partial each in S2 / S3 (:384, :406)
 NODE_WARPS = NODE_THREADS // 32
-D_SPLIT = NODE_THREADS // 2   # jslp_node_kernel.cuh:413: threads below NT / 2 normalise the pivot row, the rest the column
-U_BLOCK = 128           # jslp_node_kernel.cuh:433: the row update walks the columns in blocks of 4 x 32
+D_SPLIT = NODE_THREADS // 2   # jslp_node_kernel.cuh:453: threads below NT / 2 normalise the pivot row, the rest the column
+U_BLOCK = 128           # jslp_node_kernel.cuh:473: the row update walks the columns in blocks of 4 x 32
 PRICE_BATCH = 50        # jslp_api.cu:248: smallest partial-pricing batch; on while W - 1 > 2 x batch (:250)
 NODE_LOG_HEAD = 64      # jslp_node_kernel.cuh:34: pivot-log entries a CTA reports inline
 
