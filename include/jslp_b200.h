@@ -383,6 +383,29 @@ int jslp_pool_batch(jslp_tab *tab, const jslp_fix *fixes, const int32_t *fix_off
                     double *evaluation, int32_t *is_integral, int32_t *branch_var, double *branch_value,
                     int32_t *pivots, double *rhs, int32_t *vrow);
 
+/* The node LPs of the bounding searches behind the near-optimal variability of a MIP, DESIGN.md section 2o.  Node i is
+ * the saved snapshot (a bound tableau, jslp_bound_create) with the cost edits edits[edit_offsets[i] ..
+ * edit_offsets[i+1]) applied in order as jslp_scenario_batch applies them (kind 1 = updateCost of the label `index`,
+ * resolved against the snapshot's labels; every other kind is JSLP_E_INVALID), then the cut rows cuts[cut_offsets[i] ..
+ * cut_offsets[i+1]) appended as jslp_add_cuts appends them (labels from the snapshot's lastElementIndex), then
+ * simplex() with check_cycles and the isIntegral / getMostFractionalVar scan.  Nodes whose rows fit shared memory run
+ * one CTA each in one launch; the others, and any node whose pivot log shows a cycle or that hits the in-kernel pivot
+ * or log cap, run one after another on the single-tableau path.  The outputs are jslp_pool_batch's, per node:
+ *   status         0 optimal, 1 infeasible, 2 unbounded, 3 cycled (the cycle check fired)
+ *   evaluation     Tableau.evaluation when optimal (M[0,0] rounded to the precision), -inf when unbounded, else 0
+ *   is_integral    1 when optimal and every basic integer variable is integral
+ *   branch_var / branch_value   getMostFractionalVar when optimal and not integral, else -1 / 0
+ *   pivots         phase-1 plus phase-2 pivots
+ *   rhs, vrow      row_stride entries each at i * row_stride; for an integral node the first H + n_cuts(i) hold the
+ *                  final column 0 and row labels, otherwise they are not written
+ * row_stride must be at least the snapshot's height plus every node's cut count.  Needs a snapshot (jslp_save); on
+ * return the tableau equals it, and the scalar Tableau state and executed-pivot log are as they were.  No optional
+ * objectives (JSLP_E_UNSUPPORTED). */
+int jslp_target_batch(jslp_tab *tab, const jslp_scenario_edit *edits, const int32_t *edit_offsets, const jslp_cut *cuts,
+                      const int32_t *cut_offsets, int n_nodes, int check_cycles, int row_stride, int32_t *status,
+                      double *evaluation, int32_t *is_integral, int32_t *branch_var, double *branch_value,
+                      int32_t *pivots, double *rhs, int32_t *vrow);
+
 /* The node LPs of the feasibility searches behind a MIP conflict, DESIGN.md section 2n.  Node i is cost row 0 plus the
  * rows r >= 1 of the saved snapshot with keep[i * H + r] != 0 (H = the snapshot's height; row 0 is always kept), in
  * their original order, followed by the cut rows cuts[cut_offsets[i] .. cut_offsets[i+1]) appended as jslp_add_cuts

@@ -169,8 +169,8 @@ struct jslp_tab {
     long long node_kernel_ns = 0;  // sum over rounds of the slowest node CTA (reporting)
     unsigned long long *d_sens = nullptr;  // jslp_sensitivity's key buffers: 2 x sens_cap
     size_t sens_cap = 0;
-    // jslp_feasibility_batch / jslp_conflict_batch / jslp_scenario_batch / jslp_column_batch / jslp_pool_batch
-    // (batch_scratch): one launch's keep and integer masks, or the gathered row list and integer mask of one node, or
+    // jslp_feasibility_batch / jslp_conflict_batch / jslp_scenario_batch / jslp_column_batch / jslp_pool_batch /
+    // jslp_target_batch (batch_scratch): one launch's keep and integer masks, or the gathered row list and integer mask of one node, or
     // one chunk's offsets, resolved edits or fixings; and per-set outputs
     void *d_scratch = nullptr;
     size_t scratch_bytes = 0;

@@ -84,13 +84,16 @@ struct NodeBatchDev {
     // memory; every right-hand-side edit before every cost edit) to the restored root, solves, and writes its final
     // column 0 and row labels to out_rhs / out_vrow + n * Hcap (NODE_COLUMNS writes them too).  Not read by the other
     // modes.
-    // Pool launches (NODE_POOL, jslp_pool_batch) apply the EDIT_FIX_COL edits[edit_off[n] .. edit_off[n+1]) (device
-    // memory) to the restored root in list order, then append node n's cut rows as NODE_BRANCH does; they write column
-    // 0 and the row labels too.  The final columns go to out_rhs / out_vrow + n * Hcap.
+    // Pool launches (NODE_POOL: jslp_pool_batch, jslp_target_batch) apply edits[edit_off[n] .. edit_off[n+1]) (device
+    // memory) to the restored root: the EDIT_FIX_COL edits in list order, then, when cost_edits is set, the
+    // EDIT_COST_ROW / EDIT_COST_COL edits in list order as NODE_SCENARIO applies them; then they append node n's cut
+    // rows as NODE_BRANCH does.  They write column 0 and the row labels too.  The final columns go to out_rhs /
+    // out_vrow + n * Hcap.
     const EditDev *edits;
     const int *edit_off;
     double *out_rhs;
     int *out_vrow;
+    int cost_edits;
     int n_inline;         // > 0: cut_off_inline holds the n_inline + 1 offsets (saves a PCIe round trip)
     int cut_off_inline[NODE_INLINE_OFF + 1];
     // Row-subset launches (NODE_CONFLICT: jslp_conflict_batch, and jslp_feasibility_batch without cuts, mask or
@@ -255,7 +258,8 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
         // setRightHandSide / setCost on the restored root (DESIGN.md 2e): every edit writes column 0 or row 0 only and
         // reads columns >= 1 / rows >= 1, so the right-hand-side edits run as one pass over rows (each thread applies
         // all of them to its M[r,0] in order) and the cost edits, after them, as one pass over columns.  A fixing
-        // (DESIGN.md 2m) reads and then clears its own column of the thread's row, so it joins the row pass.
+        // (DESIGN.md 2m) reads and then clears its own column of the thread's row, so it joins the row pass.  A pool
+        // launch without cost edits (jslp_pool_batch) skips the column pass.
         int e0 = c0, ne = nc;
         if constexpr (POOL) { e0 = nb.edit_off[node]; ne = nb.edit_off[node + 1] - e0; }
         const EditDev *ed = nb.edits + e0;
@@ -271,18 +275,16 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
             row[0] = x;
         }
         __syncthreads();
-    }
-    if constexpr (SCENARIO) {
-        const EditDev *ed = nb.edits + c0;
-        for (int c = tid; c < W; c += NT) {
-            double x = Ms[c];
-            for (int k = 0; k < nc; k++) {
-                const EditDev e = ed[k];
-                if (e.kind == EDIT_COST_ROW) x = edit_axpy_add(x, e.d, Ms[(size_t)e.pos * Ws + c]);
-                else if (e.kind == EDIT_COST_COL && e.pos == c) x = edit_sub(x, e.d);
+        if (SCENARIO || nb.cost_edits)
+            for (int c = tid; c < W; c += NT) {
+                double x = Ms[c];
+                for (int k = 0; k < ne; k++) {
+                    const EditDev e = ed[k];
+                    if (e.kind == EDIT_COST_ROW) x = edit_axpy_add(x, e.d, Ms[(size_t)e.pos * Ws + c]);
+                    else if (e.kind == EDIT_COST_COL && e.pos == c) x = edit_sub(x, e.d);
+                }
+                Ms[c] = x;
             }
-            Ms[c] = x;
-        }
     }
     if constexpr (COLUMNS) {
         // the cleared columns of this CTA's mask are +0 in every row: a zero column prices at 0, so it never

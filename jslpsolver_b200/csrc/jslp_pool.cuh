@@ -51,17 +51,34 @@ struct PoolOut {
     }
 };
 
-// One region on the single-tableau path.  The caller restores the snapshot.
-static int pool_hbm(jslp_tab *t, const std::vector<EditDev> &fixes, const jslp_cut *cuts, int n_cuts, int check_cycles,
+// One node on the single-tableau path: the fixings by k_fix_columns, then the cost edits in list order with
+// jslp_update_cost's kernels (the arithmetic of k_node_batch<NODE_POOL>'s column pass), then the cut rows.  The caller
+// restores the snapshot.
+static int pool_hbm(jslp_tab *t, const EditDev *edits, int n_edits, const jslp_cut *cuts, int n_cuts, int check_cycles,
                     int i, PoolOut &o) {
     cudaStream_t s = t->ctx->stream;
     int rc = jslp_restore(t);
     if (rc) return rc;
+    std::vector<EditDev> fixes;
+    for (int k = 0; k < n_edits; k++)
+        if (edits[k].kind == EDIT_FIX_COL) fixes.push_back(edits[k]);
     if (!fixes.empty()) {
         rc = batch_scratch(t, sizeof(EditDev) * fixes.size());
         if (rc) return rc;
         CK(cudaMemcpyAsync(t->d_scratch, fixes.data(), sizeof(EditDev) * fixes.size(), cudaMemcpyHostToDevice, s));
         k_fix_columns<<<(t->H + 255) / 256, 256, 0, s>>>(t->d_T, (const EditDev *)t->d_scratch, (int)fixes.size());
+        t->ctx->launches += 1;
+        CK(cudaGetLastError());
+    }
+    for (int k = 0; k < n_edits; k++) {
+        const EditDev &e = edits[k];
+        if (e.kind == EDIT_COST_ROW)
+            k_row_axpy<<<std::max(1, (t->W + 255) / 256), 256, 0, s>>>(t->hd.M, t->hd.M + (size_t)e.pos * t->stride, e.d,
+                                                                      t->W, 1);
+        else if (e.kind == EDIT_COST_COL)
+            k_entry_sub<<<1, 1, 0, s>>>(t->hd.M + e.pos, e.d);
+        else
+            continue;
         t->ctx->launches += 1;
         CK(cudaGetLastError());
     }
@@ -83,17 +100,17 @@ static int pool_hbm(jslp_tab *t, const std::vector<EditDev> &fixes, const jslp_c
     return JSLP_OK;
 }
 
-// Regions idx[0..n) in one k_node_batch<NODE_POOL> launch.  Those whose log shows a cycle (per-phase histories, with
+// Nodes idx[0..n) in one k_node_batch<NODE_POOL> launch.  Those whose log shows a cycle (per-phase histories, with
 // check_cycles) or that hit the pivot or log cap go to redo.
-static int pool_resident(jslp_tab *t, const std::vector<EditDev> &fixes, const int32_t *fix_off, const jslp_cut *cuts,
+static int pool_resident(jslp_tab *t, const std::vector<EditDev> &edits, const int32_t *edit_off, const jslp_cut *cuts,
                          const int32_t *cut_off, const int *idx, int n, int check_cycles, PoolOut &o,
                          std::vector<int> &redo) {
     ResidentBufs &rb = t->rbufs;
     const int H0 = t->saved.H;
-    int maxc = 0, totf = 0;
+    int maxc = 0, tote = 0;
     for (int k = 0; k < n; k++) {
         maxc = std::max(maxc, cut_off[idx[k] + 1] - cut_off[idx[k]]);
-        totf += fix_off[idx[k] + 1] - fix_off[idx[k]];
+        tote += edit_off[idx[k] + 1] - edit_off[idx[k]];
     }
     NodeBatchDev nb;
     size_t smem = 0;
@@ -103,26 +120,29 @@ static int pool_resident(jslp_tab *t, const std::vector<EditDev> &fixes, const i
     if (rc) return rc;
     nb.Hcap = H0 + maxc;
     smem = node_smem_bytes(nb.Hcap, t->W, nullptr);
-    std::vector<int> foff((size_t)n + 1);
-    std::vector<EditDev> fx((size_t)std::max(1, totf));
+    std::vector<int> eoff((size_t)n + 1);
+    std::vector<EditDev> ed((size_t)std::max(1, tote));
     int f = 0;
     for (int k = 0; k < n; k++) {
-        foff[k] = f;
-        for (int h = fix_off[idx[k]]; h < fix_off[idx[k] + 1]; h++) fx[f++] = fixes[h];
+        eoff[k] = f;
+        for (int h = edit_off[idx[k]]; h < edit_off[idx[k] + 1]; h++) {
+            nb.cost_edits |= edits[h].kind == EDIT_COST_ROW || edits[h].kind == EDIT_COST_COL;
+            ed[f++] = edits[h];
+        }
     }
-    foff[n] = f;
-    // one device block per chunk: fixing offsets, fixings, final columns, final labels
-    const size_t b_fx = (sizeof(int) * (size_t)(n + 1) + 15) & ~(size_t)15;
-    const size_t b_rhs = b_fx + ((sizeof(EditDev) * (size_t)totf + 15) & ~(size_t)15);
+    eoff[n] = f;
+    // one device block per chunk: edit offsets, edits, final columns, final labels
+    const size_t b_ed = (sizeof(int) * (size_t)(n + 1) + 15) & ~(size_t)15;
+    const size_t b_rhs = b_ed + ((sizeof(EditDev) * (size_t)tote + 15) & ~(size_t)15);
     const size_t b_vrow = b_rhs + sizeof(double) * (size_t)n * nb.Hcap;
     rc = batch_scratch(t, b_vrow + sizeof(int) * (size_t)n * nb.Hcap);
     if (rc) return rc;
     char *base = (char *)t->d_scratch;
     cudaStream_t s = t->ctx->stream;
-    CK(cudaMemcpyAsync(base, foff.data(), sizeof(int) * (size_t)(n + 1), cudaMemcpyHostToDevice, s));
-    if (totf > 0) CK(cudaMemcpyAsync(base + b_fx, fx.data(), sizeof(EditDev) * (size_t)totf, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(base, eoff.data(), sizeof(int) * (size_t)(n + 1), cudaMemcpyHostToDevice, s));
+    if (tote > 0) CK(cudaMemcpyAsync(base + b_ed, ed.data(), sizeof(EditDev) * (size_t)tote, cudaMemcpyHostToDevice, s));
     nb.edit_off = (const int *)base;
-    nb.edits = (const EditDev *)(base + b_fx);
+    nb.edits = (const EditDev *)(base + b_ed);
     nb.out_rhs = (double *)(base + b_rhs); nb.out_vrow = (int *)(base + b_vrow);
     std::vector<double> rhs((size_t)n * nb.Hcap);
     std::vector<int32_t> vrow((size_t)n * nb.Hcap);
@@ -149,58 +169,113 @@ static int pool_resident(jslp_tab *t, const std::vector<EditDev> &fixes, const i
     return JSLP_OK;
 }
 
-extern "C" int jslp_pool_batch(jslp_tab *t, const jslp_fix *fixes, const int32_t *fix_offsets, const jslp_cut *cuts,
-                               const int32_t *cut_offsets, int n_nodes, int check_cycles, int row_stride,
-                               int32_t *status, double *evaluation, int32_t *is_integral, int32_t *branch_var,
-                               double *branch_value, int32_t *pivots, double *rhs, int32_t *vrow) {
-    if (!t) return fail(JSLP_E_INVALID, "tab is NULL");
-    if (n_nodes < 0 || (n_nodes > 0 && (!fix_offsets || !cut_offsets || !status || !evaluation || !is_integral ||
-                                        !branch_var || !branch_value || !pivots || !rhs || !vrow)))
-        return fail(JSLP_E_INVALID, "pool_batch: bad offsets / output arguments");
-    if (!t->saved.valid) return fail(JSLP_E_INVALID, "pool_batch needs a snapshot (jslp_save)");
-    if (t->nOpt > 0) return fail(JSLP_E_UNSUPPORTED, "pool_batch: optional objectives are not supported");
-    if (n_nodes == 0) return JSLP_OK;
-    if (fix_offsets[0] != 0 || cut_offsets[0] != 0) return fail(JSLP_E_INVALID, "pool_batch: offsets[0] must be 0");
-    const int W = t->W, H0 = t->saved.H;
-    for (int i = 0; i < n_nodes; i++) {
-        if (fix_offsets[i + 1] < fix_offsets[i] || cut_offsets[i + 1] < cut_offsets[i])
-            return fail(JSLP_E_INVALID, "pool_batch: offsets must not decrease");
-        if (H0 + cut_offsets[i + 1] - cut_offsets[i] > row_stride)
-            return fail(JSLP_E_INVALID, "pool_batch: row_stride is below a region's height (rows plus cuts)");
-    }
-    const int n_fixes = fix_offsets[n_nodes], n_cuts = cut_offsets[n_nodes];
-    if ((n_fixes > 0 && !fixes) || (n_cuts > 0 && !cuts)) return fail(JSLP_E_INVALID, "pool_batch: fixes / cuts is NULL");
-    std::vector<EditDev> fx((size_t)n_fixes);
-    for (int k = 0; k < n_fixes; k++) {
-        if (fixes[k].column < 1 || fixes[k].column >= W) return fail(JSLP_E_INVALID, "pool_batch: fixed column out of range");
-        fx[k] = EditDev{EDIT_FIX_COL, fixes[k].column, fixes[k].value};
-    }
-    for (int k = 0; k < n_cuts; k++)
-        if ((cuts[k].type != 0 && cuts[k].type != 1) || cuts[k].var_index < 0 || cuts[k].var_index >= t->saved.nVars)
-            return fail(JSLP_E_INVALID, "pool_batch: cut type must be 0 (min) or 1 (max), on a label of the snapshot");
+// The node LPs of jslp_pool_batch and jslp_target_batch: node i is the snapshot with edits[edit_off[i] ..
+// edit_off[i+1]) and the cut rows cuts[cut_off[i] .. cut_off[i+1]).  Nodes whose rows fit shared memory run in chunks
+// of k_node_batch<NODE_POOL> launches, the others and the redone ones on the single-tableau path; the tableau ends
+// equal to the snapshot, with the caller's scalar state.
+static int pool_run(jslp_tab *t, const std::vector<EditDev> &edits, const int32_t *edit_off, const jslp_cut *cuts,
+                    const int32_t *cut_off, int n_nodes, int check_cycles, PoolOut &o) {
     CK(cudaSetDevice(t->ctx->device));
-    PoolOut o{status, is_integral, branch_var, pivots, evaluation, branch_value, rhs, vrow, row_stride};
+    const int H0 = t->saved.H;
     const CallerState caller(t);
     std::vector<int> res, redo;
     int maxc = 0;
     for (int i = 0; i < n_nodes; i++) {
-        const int nc = cut_offsets[i + 1] - cut_offsets[i];
+        const int nc = cut_off[i + 1] - cut_off[i];
         if (batch_resident(t, H0 + nc)) { res.push_back(i); maxc = std::max(maxc, nc); }
         else redo.push_back(i);
     }
     int rc = JSLP_OK;
     const int chunk = batch_chunk(H0 + maxc);
     for (size_t k0 = 0; k0 < res.size() && rc == JSLP_OK; k0 += chunk)
-        rc = pool_resident(t, fx, fix_offsets, cuts, cut_offsets, res.data() + k0,
+        rc = pool_resident(t, edits, edit_off, cuts, cut_off, res.data() + k0,
                            (int)std::min<size_t>(chunk, res.size() - k0), check_cycles, o, redo);
     for (size_t k = 0; k < redo.size() && rc == JSLP_OK; k++) {
         const int i = redo[k];
-        const std::vector<EditDev> mine(fx.begin() + fix_offsets[i], fx.begin() + fix_offsets[i + 1]);
-        rc = pool_hbm(t, mine, cuts + cut_offsets[i], cut_offsets[i + 1] - cut_offsets[i], check_cycles, i, o);
+        rc = pool_hbm(t, edits.data() + edit_off[i], edit_off[i + 1] - edit_off[i], cuts + cut_off[i],
+                      cut_off[i + 1] - cut_off[i], check_cycles, i, o);
     }
     const int rc2 = jslp_restore(t);
     if (rc == JSLP_OK) rc = rc2;
     CK(cudaStreamSynchronize(t->ctx->stream));
     caller.restore(t);
     return rc;
+}
+
+// The checks jslp_pool_batch and jslp_target_batch share, with `what` naming the entry point and `node` its nodes in
+// the messages.
+static int pool_check(jslp_tab *t, const int32_t *edit_offsets, const jslp_cut *cuts, const int32_t *cut_offsets,
+                      int n_nodes, int row_stride, bool outputs, const std::string &what, const char *node) {
+    if (!t) return fail(JSLP_E_INVALID, "tab is NULL");
+    if (n_nodes < 0 || (n_nodes > 0 && (!edit_offsets || !cut_offsets || !outputs)))
+        return fail(JSLP_E_INVALID, what + ": bad offsets / output arguments");
+    if (!t->saved.valid) return fail(JSLP_E_INVALID, what + " needs a snapshot (jslp_save)");
+    if (t->nOpt > 0) return fail(JSLP_E_UNSUPPORTED, what + ": optional objectives are not supported");
+    if (n_nodes == 0) return JSLP_OK;
+    if (edit_offsets[0] != 0 || cut_offsets[0] != 0) return fail(JSLP_E_INVALID, what + ": offsets[0] must be 0");
+    for (int i = 0; i < n_nodes; i++) {
+        if (edit_offsets[i + 1] < edit_offsets[i] || cut_offsets[i + 1] < cut_offsets[i])
+            return fail(JSLP_E_INVALID, what + ": offsets must not decrease");
+        if (t->saved.H + cut_offsets[i + 1] - cut_offsets[i] > row_stride)
+            return fail(JSLP_E_INVALID, what + ": row_stride is below a " + node + "'s height (rows plus cuts)");
+    }
+    return JSLP_OK;
+}
+
+static int pool_check_cuts(const jslp_tab *t, const jslp_cut *cuts, int n_cuts, const std::string &what) {
+    for (int k = 0; k < n_cuts; k++)
+        if ((cuts[k].type != 0 && cuts[k].type != 1) || cuts[k].var_index < 0 || cuts[k].var_index >= t->saved.nVars)
+            return fail(JSLP_E_INVALID, what + ": cut type must be 0 (min) or 1 (max), on a label of the snapshot");
+    return JSLP_OK;
+}
+
+extern "C" int jslp_pool_batch(jslp_tab *t, const jslp_fix *fixes, const int32_t *fix_offsets, const jslp_cut *cuts,
+                               const int32_t *cut_offsets, int n_nodes, int check_cycles, int row_stride,
+                               int32_t *status, double *evaluation, int32_t *is_integral, int32_t *branch_var,
+                               double *branch_value, int32_t *pivots, double *rhs, int32_t *vrow) {
+    int rc = pool_check(t, fix_offsets, cuts, cut_offsets, n_nodes, row_stride,
+                        status && evaluation && is_integral && branch_var && branch_value && pivots && rhs && vrow,
+                        "pool_batch", "region");
+    if (rc || n_nodes == 0) return rc;
+    const int n_fixes = fix_offsets[n_nodes], n_cuts = cut_offsets[n_nodes];
+    if ((n_fixes > 0 && !fixes) || (n_cuts > 0 && !cuts)) return fail(JSLP_E_INVALID, "pool_batch: fixes / cuts is NULL");
+    std::vector<EditDev> fx((size_t)n_fixes);
+    for (int k = 0; k < n_fixes; k++) {
+        if (fixes[k].column < 1 || fixes[k].column >= t->W) return fail(JSLP_E_INVALID, "pool_batch: fixed column out of range");
+        fx[k] = EditDev{EDIT_FIX_COL, fixes[k].column, fixes[k].value};
+    }
+    rc = pool_check_cuts(t, cuts, n_cuts, "pool_batch");
+    if (rc) return rc;
+    PoolOut o{status, is_integral, branch_var, pivots, evaluation, branch_value, rhs, vrow, row_stride};
+    return pool_run(t, fx, fix_offsets, cuts, cut_offsets, n_nodes, check_cycles, o);
+}
+
+extern "C" int jslp_target_batch(jslp_tab *t, const jslp_scenario_edit *edits, const int32_t *edit_offsets,
+                                 const jslp_cut *cuts, const int32_t *cut_offsets, int n_nodes, int check_cycles,
+                                 int row_stride, int32_t *status, double *evaluation, int32_t *is_integral,
+                                 int32_t *branch_var, double *branch_value, int32_t *pivots, double *rhs, int32_t *vrow) {
+    int rc = pool_check(t, edit_offsets, cuts, cut_offsets, n_nodes, row_stride,
+                        status && evaluation && is_integral && branch_var && branch_value && pivots && rhs && vrow,
+                        "target_batch", "node");
+    if (rc || n_nodes == 0) return rc;
+    const int n_edits = edit_offsets[n_nodes], n_cuts = cut_offsets[n_nodes];
+    if ((n_edits > 0 && !edits) || (n_cuts > 0 && !cuts)) return fail(JSLP_E_INVALID, "target_batch: edits / cuts is NULL");
+    // updateCost resolved once against the snapshot's labels, as jslp_scenario_batch resolves it
+    CK(cudaSetDevice(t->ctx->device));
+    HostMaps m;
+    m.vrow.resize((size_t)t->saved.H);
+    m.vcol.resize((size_t)t->W);
+    cudaStream_t s = t->ctx->stream;
+    CK(cudaMemcpyAsync(m.vrow.data(), t->saved.vrow, sizeof(int) * m.vrow.size(), cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(m.vcol.data(), t->saved.vcol, sizeof(int) * m.vcol.size(), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    std::vector<EditDev> ed((size_t)n_edits);
+    for (int k = 0; k < n_edits; k++) {
+        if (edits[k].kind != 1) return fail(JSLP_E_INVALID, "target_batch: edit kind must be 1 (cost)");
+        if (!resolve_edit(m, edits[k], &ed[k])) return fail(JSLP_E_INVALID, "target_batch: unknown variable index");
+    }
+    rc = pool_check_cuts(t, cuts, n_cuts, "target_batch");
+    if (rc) return rc;
+    PoolOut o{status, is_integral, branch_var, pivots, evaluation, branch_value, rhs, vrow, row_stride};
+    return pool_run(t, ed, edit_offsets, cuts, cut_offsets, n_nodes, check_cycles, o);
 }

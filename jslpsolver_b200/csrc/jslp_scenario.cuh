@@ -13,6 +13,16 @@
 
 enum { SCEN_OPTIMAL = 0, SCEN_INFEASIBLE = 1, SCEN_UNBOUNDED = 2, SCEN_CYCLED = 3 };
 
+// Edit e (kind 0 or 1) resolved against the labels m: a right-hand-side or cost edit of the row its label is basic in,
+// or of the column it is non-basic in.  False when the label is in neither.
+static bool resolve_edit(const HostMaps &m, const jslp_scenario_edit &e, EditDev *out) {
+    const int row = m.row_of(e.index), col = row < 0 ? m.col_of(e.index) : -1;
+    if (row < 0 && col < 0) return false;
+    if (e.kind == 0) *out = row < 0 ? EditDev{EDIT_RHS_COL, col, e.difference} : EditDev{EDIT_RHS_ROW, row, e.difference};
+    else *out = row < 0 ? EditDev{EDIT_COST_COL, col, e.difference} : EditDev{EDIT_COST_ROW, row, e.difference};
+    return true;
+}
+
 // One scenario on the single-tableau path, from the private snapshot.
 static int scenario_sequential(jslp_tab *t, const jslp_scenario_edit *e, int n, int check_cycles, int32_t *status,
                                double *eval_raw, int32_t *p1, int32_t *p2, double *rhs, int32_t *vrow) {
@@ -108,10 +118,7 @@ extern "C" int jslp_scenario_batch(jslp_tab *t, const jslp_scenario_edit *edits,
             if (e.kind != 0 && e.kind != 1) return fail(JSLP_E_INVALID, "scenario_batch: edit kind must be 0 (rhs) or 1 (cost)");
             if (e.kind == 0 && k > offsets[i] && edits[k - 1].kind == 1)
                 return fail(JSLP_E_INVALID, "scenario_batch: a scenario's right-hand-side edits come before its cost edits");
-            const int row = m.row_of(e.index), col = row < 0 ? m.col_of(e.index) : -1;
-            if (row < 0 && col < 0) return fail(JSLP_E_INVALID, "scenario_batch: unknown constraint or variable index");
-            if (e.kind == 0) res[k] = row < 0 ? EditDev{EDIT_RHS_COL, col, e.difference} : EditDev{EDIT_RHS_ROW, row, e.difference};
-            else res[k] = row < 0 ? EditDev{EDIT_COST_COL, col, e.difference} : EditDev{EDIT_COST_ROW, row, e.difference};
+            if (!resolve_edit(m, e, &res[k])) return fail(JSLP_E_INVALID, "scenario_batch: unknown constraint or variable index");
         }
     const CallerState caller(t);
     rc = ensure_snapshot(t, 2);

@@ -30,11 +30,11 @@ OPTIMAL, INFEASIBLE, UNBOUNDED, CYCLED = 0, 1, 2, 3
 DEFAULT_WIDTH = 16
 
 
-def _count(name: str, x, lo: int) -> int:
+def _count(name: str, x, lo: int, what: str = WHAT) -> int:
     if isinstance(x, bool) or not isinstance(x, numbers.Integral):
-        raise ValueError(f"{WHAT}: {name}= takes an integer, not {type(x).__name__}")
+        raise ValueError(f"{what}: {name}= takes an integer, not {type(x).__name__}")
     if x < lo:
-        raise ValueError(f"{WHAT}: {name}= must be >= {lo}, not {x!r}")
+        raise ValueError(f"{what}: {name}= must be >= {lo}, not {x!r}")
     return int(x)
 
 

@@ -8,6 +8,7 @@ from . import validation
 from .conflict import Conflict as _conflict
 from .frontier import Frontier as _frontier
 from .lexicographic import Lexicographic as _lexicographic
+from .mip_variability import Variability as _variability
 from .model import Model, object_keys
 from .polyopt import Polyopt
 from .pool import Pool as _pool
@@ -92,6 +93,13 @@ class Solver:
         the plan that breaks only it (conflict.py, DESIGN.md section 2n).  `width` / `depth` tune the batching only."""
         return _conflict(self, model, max_nodes, width, depth, precision, validate)
 
+    def Variability(self, model: dict, gap=0.0, absolute_gap=0.0, variables=None, constraints=None, points=False,
+                    max_nodes=10000, width=None, precision: Optional[float] = None, validate: bool = False) -> dict:
+        """The range of every variable and slack of a MIP over all integer plans within an allowance of the optimum,
+        each end exact or bounded (mip_variability.py, DESIGN.md section 2o).  `width` tunes the batching only."""
+        return _variability(self, model, gap, absolute_gap, variables, constraints, points, max_nodes, width, precision,
+                            validate)
+
     def _instance(self, model: Any, precision: Optional[float]) -> Model:
         if isinstance(model, dict):
             options = model.get("options") or {}
@@ -165,3 +173,9 @@ def Pool(model: dict, k=10, gap=0.0, absolute_gap=0.0, precision: Optional[float
 def Conflict(model: dict, max_nodes=10000, width=None, depth=None, precision: Optional[float] = None,
              validate: bool = False) -> dict:
     return solver.Conflict(model, max_nodes, width, depth, precision, validate)
+
+
+def Variability(model: dict, gap=0.0, absolute_gap=0.0, variables=None, constraints=None, points=False,
+                max_nodes=10000, width=None, precision: Optional[float] = None, validate: bool = False) -> dict:
+    return solver.Variability(model, gap, absolute_gap, variables, constraints, points, max_nodes, width, precision,
+                              validate)

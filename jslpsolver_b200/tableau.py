@@ -840,26 +840,43 @@ class GpuTableau:
         evaluation, is_integral, branch_var / branch_value, pivots, and rhs / vrow (n x row_stride, written for
         integral regions: the final column 0 and row labels, height + len(cuts) entries).  Leaves the tableau equal to
         its snapshot."""
-        n = len(regions)
-        fix_off, cut_off = np.zeros(n + 1, dtype=np.int32), np.zeros(n + 1, dtype=np.int32)
-        for i, (fx, cs) in enumerate(regions):
-            fix_off[i + 1], cut_off[i + 1] = fix_off[i] + len(fx), cut_off[i] + len(cs)
-        fixes = (_lib.Fix * max(1, int(fix_off[-1])))()
+        fixes = (_lib.Fix * max(1, sum(len(fx) for fx, _ in regions)))()
         k = 0
         for fx, _ in regions:
             for col, value in fx:
                 fixes[k].column, fixes[k].value = int(col), float(value)
                 k += 1
-        cuts = self._cut_array([c for _, cs in regions for c in cs])
-        stride = self.height + max((len(cs) for _, cs in regions), default=0)
+        return self._node_batch(self.context.lib.jslp_pool_batch, fixes, regions, check_cycles)
+
+    def target_batch(self, nodes, check_cycles: Optional[bool] = None) -> dict:
+        """jslp_target_batch: the node LPs of the bounding searches of a MIP's near-optimal variability (DESIGN.md
+        section 2o).  nodes = [(edits, cuts), ...] with edits [(1, label, difference), ...] applied in order to the
+        saved snapshot as updateCost applies them, then the cuts appended and simplex() run as pool_batch does.
+        Returns what pool_batch returns.  Leaves the tableau equal to its snapshot."""
+        arr = (ScenarioEdit * max(1, sum(len(ed) for ed, _ in nodes)))()
+        k = 0
+        for ed, _ in nodes:
+            for kind, index, difference in ed:
+                arr[k].kind, arr[k].index, arr[k].difference = int(kind), int(index), float(difference)
+                k += 1
+        return self._node_batch(self.context.lib.jslp_target_batch, arr, nodes, check_cycles)
+
+    def _node_batch(self, fn, edits, nodes, check_cycles: Optional[bool]) -> dict:
+        """The call and outputs jslp_pool_batch and jslp_target_batch share: edits (a ctypes array) in the order of
+        nodes = [(edits of node i, cuts of node i), ...]."""
+        n = len(nodes)
+        edit_off, cut_off = np.zeros(n + 1, dtype=np.int32), np.zeros(n + 1, dtype=np.int32)
+        for i, (ed, cs) in enumerate(nodes):
+            edit_off[i + 1], cut_off[i + 1] = edit_off[i] + len(ed), cut_off[i] + len(cs)
+        cuts = self._cut_array([c for _, cs in nodes for c in cs])
+        stride = self.height + max((len(cs) for _, cs in nodes), default=0)
         status, integral, bvar, pivots = (np.empty(n, dtype=np.int32) for _ in range(4))
         evaluation, bval = np.empty(n, dtype=np.float64), np.empty(n, dtype=np.float64)
         rhs, vrow = np.zeros((n, stride), dtype=np.float64), np.zeros((n, stride), dtype=np.int32)
         cc = self._check_cycles() if check_cycles is None else int(bool(check_cycles))
-        _lib.check(self.context.lib.jslp_pool_batch(
-            self._h(), fixes, fix_off.ctypes.data, cuts, cut_off.ctypes.data, n, cc, stride, status.ctypes.data,
-            evaluation.ctypes.data, integral.ctypes.data, bvar.ctypes.data, bval.ctypes.data, pivots.ctypes.data,
-            rhs.ctypes.data, vrow.ctypes.data))
+        _lib.check(fn(self._h(), edits, edit_off.ctypes.data, cuts, cut_off.ctypes.data, n, cc, stride,
+                      status.ctypes.data, evaluation.ctypes.data, integral.ctypes.data, bvar.ctypes.data,
+                      bval.ctypes.data, pivots.ctypes.data, rhs.ctypes.data, vrow.ctypes.data))
         self._refresh_dims()
         return {"status": status, "evaluation": evaluation, "is_integral": integral, "branch_var": bvar,
                 "branch_value": bval, "pivots": pivots, "rhs": rhs, "vrow": vrow}

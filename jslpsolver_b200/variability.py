@@ -49,6 +49,36 @@ def _point(m, fixed, rhs, vrow) -> dict:
             for v in m.variables}
 
 
+def cname(c):
+    """A constraint's name in a report: its name, or its slack label for an unnamed row (a binary's `x <= 1`)."""
+    return c.name if c.name is not None else c.index
+
+
+def _select(m, variables, constraints, what: str = WHAT):
+    """(variables, constraints) of model m that variables= / constraints= name, in model order (all of them for
+    None); raises ValueError for a malformed list or an unknown name."""
+    for arg, names in (("variables", variables), ("constraints", constraints)):
+        if names is not None and (isinstance(names, (str, bytes, dict)) or not hasattr(names, "__iter__")):
+            raise ValueError(f"{what}: {arg}= takes a list of names, not {type(names).__name__}")
+    by_id = {v.id: v for v in m.variables}
+    shown = list(m.variables)
+    if variables is not None:
+        variables = list(variables)
+        for vid in variables:
+            if vid not in by_id:
+                raise ValueError(f"{what}: no variable named {vid!r}")
+        shown = [v for v in m.variables if v.id in set(variables)]
+    rows = list(m.constraints)
+    if constraints is not None:
+        constraints = list(constraints)
+        known = {cname(c) for c in m.constraints}
+        for name in constraints:
+            if name not in known:
+                raise ValueError(f"{what}: no constraint named {name!r}")
+        rows = [c for c in m.constraints if cname(c) in set(constraints)]
+    return shown, rows
+
+
 def compute(solution, variables=None, constraints=None, points=False, gap=0.0, absolute_gap=0.0) -> dict:
     """Solution.variability(): see the module docstring."""
     _check(solution, WHAT)
@@ -58,26 +88,7 @@ def compute(solution, variables=None, constraints=None, points=False, gap=0.0, a
     if any(m.unrestrictedVariables.values()):
         raise ValueError(f"{WHAT} does not support unrestricted variables: re-solving from an optimum where one is "
                          "basic and negative starts with phase-1 pivots, which can end 'infeasible'")
-    for what, names in (("variables", variables), ("constraints", constraints)):
-        if names is not None and (isinstance(names, (str, bytes, dict)) or not hasattr(names, "__iter__")):
-            raise ValueError(f"{WHAT}: {what}= takes a list of names, not {type(names).__name__}")
-    by_id = {v.id: v for v in m.variables}
-    shown = list(m.variables)
-    if variables is not None:
-        variables = list(variables)
-        for vid in variables:
-            if vid not in by_id:
-                raise ValueError(f"{WHAT}: no variable named {vid!r}")
-        shown = [v for v in m.variables if v.id in set(variables)]
-    cname = lambda c: c.name if c.name is not None else c.index  # noqa: E731
-    rows = list(m.constraints)
-    if constraints is not None:
-        constraints = list(constraints)
-        known = {cname(c) for c in m.constraints}
-        for name in constraints:
-            if name not in known:
-                raise ValueError(f"{WHAT}: no constraint named {name!r}")
-        rows = [c for c in m.constraints if cname(c) in set(constraints)]
+    shown, rows = _select(m, variables, constraints)
     fixed = m.presolveResult.fixedVariables if m.presolveResult is not None else {}
 
     rhs, cost, vrow, vcol = t.final_state()
