@@ -504,6 +504,22 @@ typedef struct {
 
 int jslp_branch_and_cut(jslp_tab *root, const jslp_bnb_opts *opts, jslp_bnb_status *out,
                         jslp_cut *best_cuts, int best_cuts_cap);
+/* What-if scenarios of a MIP, DESIGN.md section 2p: scenario s is jslp_branch_and_cut's default service (service 0)
+ * over the tab's current tableau with rows 1.. of column 0 replaced by col0[s * H + r] and row 0 by row0[s * W + c]
+ * (H x W = the tab's size), every tree committed in its own best-first order.  Each round evaluates the next
+ * opts->max_spec_batch (0 = 16) open nodes of every live tree together, in k_node_batch launches that carry the nodes
+ * of all trees.  A tableau beyond shared memory runs its scenarios one after another through jslp_branch_and_cut.
+ * Without integer variables each scenario is its root LP, as jslp_simplex solves it.  Per scenario:
+ *   status         feasible, bounded, is_integral, iterations, n_best_cuts, pivots, evaluation and best_possible_eval
+ *                  as jslp_branch_and_cut reports them for that scenario; rounds, nodes_evaluated and nodes_pruned
+ *                  count this call's own rounds and node LPs (jslp_branch_and_cut's HBM paths also prune inside a
+ *                  round); status[0].kernel_launches counts the launches of the whole call
+ *   rhs, vrow      row_stride entries each at s * row_stride: the final column 0 and row labels, height[s] of them
+ * row_stride must be at least H plus two cuts per integer variable.  opts->service, keep_solutions, timeout_ms and
+ * n_ranks > 1, useMIRCuts and optional objectives are JSLP_E_UNSUPPORTED.  On return the tab's tableau and labels,
+ * snapshot, scalar Tableau state, node log and stored solutions are as they were. */
+int jslp_bnb_batch(jslp_tab *tab, const double *col0, const double *row0, int n_scenarios, const jslp_bnb_opts *opts,
+                   int row_stride, jslp_bnb_status *status, double *rhs, int32_t *vrow, int32_t *height);
 /* Per-node trace of the last branch_and_cut: 8 doubles per committed node
  * (iteration, nCuts, feasible, evaluation, integral(-1/0/1), branchVar, branchValue, pivots). */
 int jslp_bnb_node_log(jslp_tab *root, double *entries, int64_t cap, int64_t *n);

@@ -122,6 +122,7 @@ SYMBOLS = [
     ("jslp_target_batch", C.c_int, [P, P, P, P, P, C.c_int, C.c_int, C.c_int, P, P, P, P, P, P, P, P]),
     ("jslp_conflict_batch", C.c_int, [P, P, P, P, P, C.c_int, C.c_int, P, P, P, P, P, P, P]),
     ("jslp_branch_and_cut", C.c_int, [P, C.POINTER(BnbOpts), C.POINTER(BnbStatus), P, C.c_int]),
+    ("jslp_bnb_batch", C.c_int, [P, P, P, C.c_int, C.POINTER(BnbOpts), C.c_int, P, P, P, P]),
     ("jslp_bnb_node_log", C.c_int, [P, P, C.c_int64, C.POINTER(C.c_int64)]),
     ("jslp_bnb_solution", C.c_int, [P, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_int32), P, P, C.c_int]),
     ("jslp_comm_unique_id", C.c_int, [P]),

@@ -63,9 +63,8 @@ struct Snapshot {  // per-batch restart point for cycle rewind
     int rowcap = 0;
 };
 
-struct NodeLogEntry {
-    double v[8];
-};
+#include "jslp_frontier.h"
+using jslp_bnb::NodeLogEntry;
 
 // Host/device staging for batches of shared-memory-resident node LPs (k_node_batch).
 // Buffers of the shared-memory-resident node path.  Inputs (cut lists) and outputs (NodeOut records)
@@ -1384,3 +1383,4 @@ extern "C" int jslp_pivot_log(jslp_tab *t, int32_t *entries, int cap, int *n) {
 #include "jslp_cone.cuh"
 #include "jslp_pool.cuh"
 #include "jslp_conflict.cuh"
+#include "jslp_forest.cuh"

@@ -473,24 +473,23 @@ extern "C" int jslp_branch_and_cut(jslp_tab *t, const jslp_bnb_opts *opts, jslp_
     const double timeout_ms = opts->timeout_ms > 0 ? opts->timeout_ms : 0;  // branch-and-cut.ts:61-63
     auto time_up = [&] { return timeout_ms > 0 && ms_since(t_start) >= timeout_ms; };
 
-    Frontier branches;
-    int iterations = 0, rounds = 0;
-    const double tolerance = opts->tolerance;
+    Tree tree(t->nOpt);
+    Frontier &branches = tree.branches;
+    const int &iterations = tree.iterations;
+    const double &bestEvaluation = tree.bestEvaluation;
+    int rounds = 0;
     const int check_cycles = opts->check_cycles;
-    bool toleranceFlag = true, timed_out = false;
-    double bestEvaluation = INFINITY;
-    std::unique_ptr<Branch> bestBranch, lastCommitted;
-    std::vector<double> bestOpt((size_t)t->nOpt, INFINITY);
-    int64_t pivots = 0, nodes = 0, pruned = 0;
+    bool timed_out = false;
+    int64_t nodes = 0, pruned = 0;
     t->node_log.clear();
     t->solutions.clear();
     t->saved.valid = false;
     t->isIntegralFlag = 0;
     t->slot_pivots = 0; t->slot_ms = 0; t->slot_bytes = 0;
-    bool early_return = false;
     int K = opts->max_spec_batch > 0 ? opts->max_spec_batch : 16;  // any width commits in the same order
     std::vector<double> wire;
     RoundExchange ex{opts, n_ranks, {}, 0};
+    const Tree::Rule rule{opts->tolerance, opts->is_minimization, t->nOpt, opts->max_nodes};
 
     // keep_solutions (branch-and-cut.ts:143-153): the incumbent's tableau state, as generateSolutionSet reads it.
     // Node evaluators return summaries only, so the node is solved once more in place (incumbents are rare).
@@ -508,78 +507,21 @@ extern "C" int jslp_branch_and_cut(jslp_tab *t, const jslp_bnb_opts *opts, jslp_
         return JSLP_OK;
     };
 
-    // commits one evaluated node exactly like one iteration of branch-and-cut.ts:89-192
-    auto commit = [&](std::unique_ptr<Branch> active) -> int {
-        const NodeEval ev = active->ev;
-        iterations++;
-        t->feasible = ev.feasible; t->bounded = ev.bounded;
-        if (ev.feasible) t->evaluation = ev.evaluation;
-        if (ev.optimal) {  // setEvaluation + simplexIters (tableau.ts:420-430, simplex.ts:266-267)
-            if (t->simplexIters == 0) t->bestPossibleEval = ev.n_optimal >= 0 ? ev.first_eval : ev.evaluation;
-            t->simplexIters += ev.n_optimal >= 0 ? ev.n_optimal : 1;
-        }
-        NodeLogEntry nl;
-        nl.v[0] = iterations; nl.v[1] = (double)active->cuts.size(); nl.v[2] = ev.feasible;
-        nl.v[3] = t->evaluation; nl.v[4] = -1; nl.v[5] = -1; nl.v[6] = 0; nl.v[7] = ev.pivots;
-        auto done = [&](std::unique_ptr<Branch> keep) {
-            t->node_log.push_back(nl);
-            lastCommitted = std::move(keep);
-        };
-        if (!ev.feasible) { done(std::move(active)); return 0; }
-        const double evaluation = ev.evaluation;
-        if (evaluation > bestEvaluation) { done(std::move(active)); return 0; }
-        if (evaluation == bestEvaluation) {  // branch-and-cut.ts:107-127
-            bool worse = true;
-            for (int o = 0; o < t->nOpt; o++) {
-                if (ev.opt0[o] > bestOpt[o]) break;
-                if (ev.opt0[o] < bestOpt[o]) { worse = false; break; }
-            }
-            if (worse) { done(std::move(active)); return 0; }
-        }
-        if (ev.is_integral) {
-            nl.v[4] = 1;
-            t->isIntegralFlag = 1;
-            if (iterations == 1) { t->node_log.push_back(nl); early_return = true; return 1; }
-            bestEvaluation = evaluation;
-            for (int o = 0; o < t->nOpt; o++) bestOpt[o] = ev.opt0[o];
-            t->node_log.push_back(nl);
-            bestBranch.reset(new Branch{active->relaxedEvaluation, active->cuts, NodeEval()});
-            if (opts->keep_solutions) {
-                int rc = store_solution(*active);
-                if (rc) return rc;
-            }
-            lastCommitted = std::move(active);
-        } else {
-            if (iterations == 1) {  // snapshot = optimal root tableau (branch-and-cut.ts:155-157)
-                int rc = jslp_save(t);
-                if (rc) return rc;
-            }
-            const int varIndex = ev.branch_var;
-            const double value = ev.branch_value;
-            nl.v[4] = 0; nl.v[5] = varIndex; nl.v[6] = value;
-            std::unique_ptr<Branch> high(new Branch{evaluation, {}, NodeEval()}), low(new Branch{evaluation, {}, NodeEval()});
-            for (const jslp_cut &cut : active->cuts) {  // branch-and-cut.ts:166-179
-                if (cut.var_index == varIndex) {
-                    if (cut.type == 0) low->cuts.push_back(cut); else high->cuts.push_back(cut);
-                } else {
-                    high->cuts.push_back(cut);
-                    low->cuts.push_back(cut);
-                }
-            }
-            high->cuts.push_back(jslp_cut{0, varIndex, std::ceil(value)});
-            low->cuts.push_back(jslp_cut{1, varIndex, std::floor(value)});
-            branches.push(std::move(high));
-            branches.push(std::move(low));
-            done(std::move(active));
-        }
-        return 0;
+    // The tree's scalars are the tab's: node evaluations on the single-tableau path and keep_solutions' re-solves
+    // change the tab's between commits, and the commit reads them (Tableau.evaluation of an infeasible node's log row).
+    auto load = [&] {
+        tree.feasible = t->feasible; tree.bounded = t->bounded; tree.evaluation = t->evaluation;
+        tree.bestPossibleEval = t->bestPossibleEval; tree.simplexIters = t->simplexIters; tree.isIntegral = t->isIntegralFlag;
+    };
+    auto store = [&] {
+        t->feasible = tree.feasible; t->bounded = tree.bounded; t->evaluation = tree.evaluation;
+        t->bestPossibleEval = tree.bestPossibleEval; t->simplexIters = tree.simplexIters; t->isIntegralFlag = tree.isIntegral;
     };
 
     double eval_ms = 0, commit_ms = 0, root_ms = 0, final_ms = 0;
     t->node_kernel_ns = 0;
-    branches.push(std::unique_ptr<Branch>(new Branch{-INFINITY, {}, NodeEval()}));
     bool stop = false;
-    while (!stop && !branches.empty() && toleranceFlag) {
+    while (!stop && !branches.empty() && tree.toleranceFlag) {
         // ---- speculate: evaluate the next K un-evaluated open nodes in pop order ---------------
         const int width = iterations == 0 ? 1 : K;  // the root decides everything: alone
         std::vector<Frontier::Entry> taken;
@@ -666,21 +608,20 @@ extern "C" int jslp_branch_and_cut(jslp_tab *t, const jslp_bnb_opts *opts, jslp_
         }
 
         // ---- commit sequentially in the reference's exact order ---------------------------------
-        while (!branches.empty() && toleranceFlag) {
-            if (opts->max_nodes > 0 && iterations >= opts->max_nodes) { stop = true; break; }
-            if (n_ranks > 1 ? round_time_up : time_up()) { timed_out = true; stop = true; break; }
-            const double acceptableThreshold = opts->is_minimization ? t->bestPossibleEval * (1 + tolerance)
-                                                                     : t->bestPossibleEval * (1 - tolerance);
-            // the reference checks the tolerance BEFORE popping, and still processes that pop
-            const bool tolHit = tolerance > 0 && bestEvaluation < acceptableThreshold;
-            if (branches.h[0].b->relaxedEvaluation <= bestEvaluation && !branches.h[0].b->ev.valid) break;  // next round
-            if (tolHit) toleranceFlag = false;
-            Frontier::Entry e = branches.pop_entry();
-            if (e.b->relaxedEvaluation > bestEvaluation) continue;
-            pivots += e.b->ev.pivots;
-            int rc = commit(std::move(e.b));
-            if (rc < 0) return rc;
-            if (rc == 1) { stop = true; break; }
+        for (;;) {
+            load();
+            const Tree::Step st = tree.step(rule, [&] { return n_ranks > 1 ? round_time_up : time_up(); });
+            store();
+            if (st == Tree::DONE || st == Tree::ROUND) break;
+            if (st == Tree::LIMIT || st == Tree::EARLY) { stop = true; break; }
+            if (st == Tree::TIMED_OUT) { timed_out = true; stop = true; break; }
+            if (st == Tree::SNAPSHOT) {  // snapshot = optimal root tableau (branch-and-cut.ts:155-157)
+                int rc = jslp_save(t);
+                if (rc) return rc;
+            } else if (st == Tree::INCUMBENT && opts->keep_solutions) {
+                int rc = store_solution(*tree.lastCommitted);
+                if (rc) return rc;
+            }
         }
         commit_ms += ms_since(t_commit);
     }
@@ -688,8 +629,10 @@ extern "C" int jslp_branch_and_cut(jslp_tab *t, const jslp_bnb_opts *opts, jslp_
     // Final tableau: the reference re-solves the winner (branch-and-cut.ts:195-197); without a
     // winner it is left at the last evaluated node.  In place on the HBM path.
     int n_best = 0;
-    if (!early_return) {
-        const Branch *fin = bestBranch ? bestBranch.get() : lastCommitted.get();
+    int64_t pivots = tree.pivots;
+    const std::unique_ptr<Branch> &bestBranch = tree.bestBranch;
+    if (!tree.early_return) {
+        const Branch *fin = bestBranch ? bestBranch.get() : tree.lastCommitted.get();
         if (fin && (bestBranch || iterations > 1)) {
             const auto t_fin = now();
             NodeEval ev;
@@ -709,6 +652,7 @@ extern "C" int jslp_branch_and_cut(jslp_tab *t, const jslp_bnb_opts *opts, jslp_
         }
     }
     t->bncIterations = iterations;
+    t->node_log = std::move(tree.node_log);
 
     float ms = 0.f;
     CK(cudaEventRecord(ctx->ev1, ctx->stream));

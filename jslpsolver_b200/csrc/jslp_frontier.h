@@ -7,6 +7,8 @@
 // ranks all-gather per node.
 #pragma once
 
+#include <cmath>
+#include <cstdint>
 #include <cstring>
 #include <memory>
 #include <utility>
@@ -70,6 +72,125 @@ struct Frontier {
             i = m;
         }
         return top;
+    }
+};
+
+// One committed node of the trace jslp_bnb_node_log reads: iteration, nCuts, feasible, evaluation, integral (-1/0/1),
+// branchVar, branchValue, pivots.
+struct NodeLogEntry {
+    double v[8];
+};
+
+// One tree of the default branch-and-cut service (branch-and-cut.ts:54-199): its frontier, its incumbent and the
+// Tableau scalars the reference's loop reads and writes.  step() is one pass of that loop's body (:76-192) over a node
+// whose LP result is cached in Branch::ev; jslp_branch_and_cut and jslp_bnb_batch both commit through it.
+struct Tree {
+    Frontier branches;
+    int iterations = 0;
+    bool toleranceFlag = true, early_return = false;
+    double bestEvaluation = INFINITY;
+    std::unique_ptr<Branch> bestBranch, lastCommitted;
+    std::vector<double> bestOpt;
+    // Tableau.feasible / bounded / evaluation / bestPossibleEval / simplexIters / __isIntegral
+    int feasible = 1, bounded = 1, simplexIters = 0, isIntegral = 0;
+    double evaluation = 0, bestPossibleEval = 0;
+    std::vector<NodeLogEntry> node_log;
+    int64_t pivots = 0;  // pivots of the committed nodes
+
+    struct Rule {
+        double tolerance;
+        int is_minimization, nOpt;
+        int64_t max_nodes;  // 0 = none
+    };
+    enum Step {
+        DONE,       // the loop condition fails: the frontier is empty or the tolerance was reached
+        ROUND,      // the next node to pop has no cached result: evaluate another round first
+        LIMIT,      // max_nodes nodes are committed
+        TIMED_OUT,  // time_up() said so before the pop
+        EARLY,      // the root was integral: the reference returns at once (:134-137)
+        NEXT,       // a node was popped (and committed unless the incumbent skips it)
+        SNAPSHOT,   // the root was committed fractional: the caller snapshots the tableau now (:155-157)
+        INCUMBENT,  // a new incumbent: lastCommitted is it (keep_solutions stores it here, :143-153)
+    };
+
+    explicit Tree(int nOpt = 0) : bestOpt((size_t)nOpt, INFINITY) {
+        branches.push(std::unique_ptr<Branch>(new Branch{-INFINITY, {}, NodeEval()}));
+    }
+
+    template <typename TimeUp>
+    Step step(const Rule &r, TimeUp time_up) {
+        if (branches.empty() || !toleranceFlag) return DONE;
+        if (r.max_nodes > 0 && iterations >= r.max_nodes) return LIMIT;
+        if (time_up()) return TIMED_OUT;
+        const double acceptableThreshold = r.is_minimization ? bestPossibleEval * (1 + r.tolerance)
+                                                             : bestPossibleEval * (1 - r.tolerance);
+        // the reference checks the tolerance BEFORE popping, and still processes that pop
+        const bool tolHit = r.tolerance > 0 && bestEvaluation < acceptableThreshold;
+        if (branches.h[0].b->relaxedEvaluation <= bestEvaluation && !branches.h[0].b->ev.valid) return ROUND;
+        if (tolHit) toleranceFlag = false;
+        Frontier::Entry e = branches.pop_entry();
+        if (e.b->relaxedEvaluation > bestEvaluation) return NEXT;
+        pivots += e.b->ev.pivots;
+        return commit(std::move(e.b), r.nOpt);
+    }
+
+  private:
+    Step commit(std::unique_ptr<Branch> active, int nOpt) {
+        const NodeEval ev = active->ev;
+        iterations++;
+        feasible = ev.feasible; bounded = ev.bounded;
+        if (ev.feasible) evaluation = ev.evaluation;
+        if (ev.optimal) {  // setEvaluation + simplexIters (tableau.ts:420-430, simplex.ts:266-267)
+            if (simplexIters == 0) bestPossibleEval = ev.n_optimal >= 0 ? ev.first_eval : ev.evaluation;
+            simplexIters += ev.n_optimal >= 0 ? ev.n_optimal : 1;
+        }
+        NodeLogEntry nl;
+        nl.v[0] = iterations; nl.v[1] = (double)active->cuts.size(); nl.v[2] = ev.feasible;
+        nl.v[3] = evaluation; nl.v[4] = -1; nl.v[5] = -1; nl.v[6] = 0; nl.v[7] = ev.pivots;
+        auto done = [&](std::unique_ptr<Branch> keep) {
+            node_log.push_back(nl);
+            lastCommitted = std::move(keep);
+        };
+        if (!ev.feasible) { done(std::move(active)); return NEXT; }
+        const double value = ev.evaluation;
+        if (value > bestEvaluation) { done(std::move(active)); return NEXT; }
+        if (value == bestEvaluation) {  // branch-and-cut.ts:107-127
+            bool worse = true;
+            for (int o = 0; o < nOpt; o++) {
+                if (ev.opt0[o] > bestOpt[o]) break;
+                if (ev.opt0[o] < bestOpt[o]) { worse = false; break; }
+            }
+            if (worse) { done(std::move(active)); return NEXT; }
+        }
+        if (ev.is_integral) {
+            nl.v[4] = 1;
+            isIntegral = 1;
+            if (iterations == 1) { node_log.push_back(nl); early_return = true; return EARLY; }
+            bestEvaluation = value;
+            for (int o = 0; o < nOpt; o++) bestOpt[o] = ev.opt0[o];
+            node_log.push_back(nl);
+            bestBranch.reset(new Branch{active->relaxedEvaluation, active->cuts, NodeEval()});
+            lastCommitted = std::move(active);
+            return INCUMBENT;
+        }
+        const int varIndex = ev.branch_var;
+        nl.v[4] = 0; nl.v[5] = varIndex; nl.v[6] = ev.branch_value;
+        std::unique_ptr<Branch> high(new Branch{value, {}, NodeEval()}), low(new Branch{value, {}, NodeEval()});
+        for (const jslp_cut &cut : active->cuts) {  // branch-and-cut.ts:166-179
+            if (cut.var_index == varIndex) {
+                if (cut.type == 0) low->cuts.push_back(cut); else high->cuts.push_back(cut);
+            } else {
+                high->cuts.push_back(cut);
+                low->cuts.push_back(cut);
+            }
+        }
+        high->cuts.push_back(jslp_cut{0, varIndex, std::ceil(ev.branch_value)});
+        low->cuts.push_back(jslp_cut{1, varIndex, std::floor(ev.branch_value)});
+        branches.push(std::move(high));
+        branches.push(std::move(low));
+        const bool root = iterations == 1;
+        done(std::move(active));
+        return root ? SNAPSHOT : NEXT;
     }
 };
 

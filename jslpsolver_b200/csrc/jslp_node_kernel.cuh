@@ -47,6 +47,8 @@ enum NodeMode : int {
     NODE_POOL = 4,      // one region of a solution-pool search per CTA: fixed columns, then cut rows (jslp_pool_batch)
     NODE_CONFLICT = 5,  // one row subset of the root per CTA, then cut rows, phase 1 only, and the integrality scan
                         // over an integer mask (jslp_conflict_batch; jslp_feasibility_batch without cuts or mask)
+    NODE_FOREST = 6,    // the roots and nodes of many branch-and-cut trees at once (jslp_bnb_batch): each CTA's own
+                        // column 0 and row 0 over the root, or each node restored from its tree's root slot
 };
 
 // One resolved scenario edit (DESIGN.md 2e): where updateRightHandSide / updateCost (dynamic-modification.ts:78-160)
@@ -104,6 +106,17 @@ struct NodeBatchDev {
     // other modes.
     const uint32_t *int_keep;
     int int_words;
+    // Forest launches (NODE_FOREST, jslp_bnb_batch).  Tree s owns root slot s: slot_M + s * slot_pitch (H0 rows at
+    // root_stride), slot_vrow + s * H0 and slot_vcol + s * W.  A root launch (col0 set) restores rootM, writes
+    // col0 + s * H0 over rows 1.. of column 0 and row0 + s * W over row 0 for s = root_of[n], solves, and writes its
+    // whole final tableau and labels to slot s.  A node launch (col0 null) restores slot root_of[n] and appends node n's cut rows
+    // as NODE_BRANCH does.  Either writes column 0 and the row labels to out_rhs / out_vrow + n * Hcap when out_rhs is
+    // set.  Not read by the other modes.
+    double *slot_M;
+    int *slot_vrow, *slot_vcol;
+    size_t slot_pitch;
+    const int *root_of;
+    const double *col0, *row0;
 };
 
 constexpr int NODE_THREADS = 256;
@@ -172,7 +185,7 @@ struct NodePart {    // per-warp partial results of a scan
 template <int MODE>
 __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, const __grid_constant__ NodeBatchDev nb) {
     constexpr bool SCENARIO = MODE == NODE_SCENARIO, COLUMNS = MODE == NODE_COLUMNS;
-    constexpr bool POOL = MODE == NODE_POOL, CONFLICT = MODE == NODE_CONFLICT;
+    constexpr bool POOL = MODE == NODE_POOL, CONFLICT = MODE == NODE_CONFLICT, FOREST = MODE == NODE_FOREST;
     extern __shared__ __align__(16) unsigned char smraw[];
     __shared__ TabDev T;
     __shared__ SelSmem sel;
@@ -190,6 +203,9 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
     long long t_start = 0;
     if (tid == 0) t_start = globaltimer_ns();
     const int H0 = nb.H0, Ws = nb.Ws;
+    // a forest node restores its tree's root slot; every other launch, and a forest root, the launch's root
+    const bool from_slot = FOREST && nb.col0 == nullptr;
+    const size_t tree = from_slot ? (size_t)nb.root_of[node] : 0;
 
     // rows live in Hcap + 1 slots: the normalised pivot row is written to the spare slot and the slot
     // table is swapped, so nobody waits for the old pivot row to be overwritten in place.  Ws is even:
@@ -232,7 +248,8 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
     __syncthreads();
     for (int r = tid; r < H0k; r += NT) {
         const int src = CONFLICT ? slot[r] : r;
-        tma_bulk_g2s(Ms + (size_t)r * Ws, nb.rootM + (size_t)src * nb.root_stride, (uint32_t)(Ws * sizeof(double)), &s_bar);
+        const double *rootM = from_slot ? nb.slot_M + tree * nb.slot_pitch : nb.rootM;
+        tma_bulk_g2s(Ms + (size_t)r * Ws, rootM + (size_t)src * nb.root_stride, (uint32_t)(Ws * sizeof(double)), &s_bar);
     }
     // the cut list may live in mapped host memory: one PCIe round trip, overlapped with the restore
     int c0, nc;
@@ -243,8 +260,9 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
     const double prec = T.prec;
     int *vcol = T.vcol;
     for (int h = tid; !SCENARIO && !COLUMNS && h < nc; h += NT) cutS[h] = nb.cuts[c0 + h];
-    for (int r = tid; r < H0k; r += NT) vrow[r] = __ldg(nb.root_vrow + (CONFLICT ? slot[r] : r));
-    for (int c = tid; c < W; c += NT) vcol[c] = __ldg(nb.root_vcol + c);
+    for (int r = tid; r < H0k; r += NT)
+        vrow[r] = __ldg((from_slot ? nb.slot_vrow + tree * H0 : nb.root_vrow) + (CONFLICT ? slot[r] : r));
+    for (int c = tid; c < W; c += NT) vcol[c] = __ldg((from_slot ? nb.slot_vcol + tree * W : nb.root_vcol) + c);
     if (!CONFLICT)
         for (int r = tid; r < nb.Hcap; r += NT) slot[r] = r;
     const int Hn = (SCENARIO || COLUMNS) ? H0k : H0k + nc;
@@ -254,6 +272,16 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
     if (CONFLICT)  // nobody reads slot until the barrier after the cut rows
         for (int r = tid; r < nb.Hcap; r += NT) slot[r] = r;
     if (tid == 0) tl1 = globaltimer_ns() - t_start;
+    if constexpr (FOREST) {
+        // a forest root: the tree's right-hand sides and costs are written over the base's (DESIGN.md 2p); rows 1.. of
+        // column 0 and row 0 are disjoint, and the next reader waits at the barrier after the (absent) cut rows
+        if (nb.col0 != nullptr) {
+            const size_t s = (size_t)nb.root_of[node];
+            const double *c0 = nb.col0 + s * H0, *r0 = nb.row0 + s * W;
+            for (int r = 1 + tid; r < H0; r += NT) Ms[(size_t)r * Ws] = c0[r];
+            for (int c = tid; c < W; c += NT) Ms[c] = r0[c];
+        }
+    }
     if constexpr (SCENARIO || POOL) {
         // setRightHandSide / setCost on the restored root (DESIGN.md 2e): every edit writes column 0 or row 0 only and
         // reads columns >= 1 / rows >= 1, so the right-hand-side edits run as one pass over rows (each thread applies
@@ -526,8 +554,8 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
     // isIntegral / most fractional variable over the final RHS column
     for (int r = tid; r < Hn; r += NT) rhs[r] = Ms[(size_t)slot[r] * Ws];
     __syncthreads();
-    if constexpr (SCENARIO || COLUMNS || POOL || CONFLICT)
-        if (!CONFLICT || nb.out_rhs != nullptr)  // a row-subset launch writes them only when asked
+    if constexpr (SCENARIO || COLUMNS || POOL || CONFLICT || FOREST)
+        if (!(CONFLICT || FOREST) || nb.out_rhs != nullptr)  // row-subset and forest launches write them only when asked
             for (int r = tid; r < Hn; r += NT) {
                 nb.out_rhs[(size_t)node * nb.Hcap + r] = rhs[r];
                 nb.out_vrow[(size_t)node * nb.Hcap + r] = vrow[r];
@@ -553,6 +581,17 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
         for (int r = tid; r < Hn; r += NT) nb.wb_vrow[r] = vrow[r];
         for (int c = tid; c < W; c += NT) nb.wb_vcol[c] = vcol[c];
     }
+    if constexpr (FOREST)
+        if (nb.col0 != nullptr) {  // a forest root: its final tableau becomes its tree's snapshot (jslp_save)
+            const size_t s = (size_t)nb.root_of[node];
+            double *dst = nb.slot_M + s * nb.slot_pitch;
+            for (int r = warp; r < Hn; r += NW) {
+                const double *row = Ms + (size_t)slot[r] * Ws;
+                for (int c = lane; c < W; c += 32) dst[(size_t)r * nb.root_stride + c] = row[c];
+            }
+            for (int r = tid; r < Hn; r += NT) nb.slot_vrow[s * H0 + r] = vrow[r];
+            for (int c = tid; c < W; c += NT) nb.slot_vcol[s * W + c] = vcol[c];
+        }
     if (tid == 0) {
         NodeResult r;
         r.status = s_fin[0]; r.p1 = s_fin[1]; r.p2 = s_fin[2]; r.log_n = s_fin[3]; r.overflow = s_fin[4];

@@ -20,30 +20,30 @@ WHAT = "scenarios()"
 PICK = "give {'min': ..., 'max': ...}"
 
 
-def _number(x, what):
+def _number(x, what, caller=WHAT):
     if isinstance(x, bool) or not isinstance(x, (int, float)) or not math.isfinite(x):
-        raise ValueError(f"{WHAT}: {what} must be a finite number, not {x!r}")
+        raise ValueError(f"{caller}: {what} must be a finite number, not {x!r}")
     return x
 
 
-def _entries(spec, key):
+def _entries(spec, key, caller=WHAT):
     part = spec.get(key)
     if part is None:
         return []
     if not isinstance(part, dict):
-        raise ValueError(f"{WHAT}: {key!r} must be a dict of name -> value, not {type(part).__name__}")
+        raise ValueError(f"{caller}: {key!r} must be a dict of name -> value, not {type(part).__name__}")
     return list(part.items())
 
 
-def edits_of(m, spec) -> list:
+def edits_of(m, spec, what=WHAT) -> list:
     """[(kind, index, difference), ...]: what the sequential path passes to Tableau.updateRightHandSide (kind 0, the
     constraint's slack index) and Tableau.updateCost (kind 1, the variable's index) for one scenario spec, in order.
-    The model is not changed."""
+    The model is not changed.  `what` names the caller in the errors."""
     if not isinstance(spec, dict):
-        raise ValueError(f"{WHAT}: a scenario is a dict with 'rhs' and / or 'cost', not {type(spec).__name__}")
+        raise ValueError(f"{what}: a scenario is a dict with 'rhs' and / or 'cost', not {type(spec).__name__}")
     extra = [k for k in spec if k not in ("rhs", "cost")]
     if extra:
-        raise ValueError(f"{WHAT}: unknown scenario key(s) {extra}: a scenario has 'rhs' and 'cost'")
+        raise ValueError(f"{what}: unknown scenario key(s) {extra}: a scenario has 'rhs' and 'cost'")
     by_index = {c.index: c for c in m.constraints}
     out, rhs, cost = [], {}, {}  # rhs / cost: the values the edits so far assigned (the Model API assigns them)
 
@@ -56,24 +56,24 @@ def edits_of(m, spec) -> list:
             rhs[c] = value
             out.append((0, c.index, float(difference)))
 
-    for name, value in _entries(spec, "rhs"):
+    for name, value in _entries(spec, "rhs", what):
         if isinstance(value, dict):
             if not value:
-                raise ValueError(f"{WHAT}: constraint {name!r}: the dict needs a 'min' and / or a 'max' key")
+                raise ValueError(f"{what}: constraint {name!r}: the dict needs a 'min' and / or a 'max' key")
             for side, v in value.items():
                 if side not in ("min", "max"):
-                    raise ValueError(f"{WHAT}: constraint {name!r}: side must be 'min' or 'max', not {side!r}")
-                labels = _constraint_rows(m, name, side, WHAT, PICK)[0]
-                set_rhs(by_index[labels[0]], _number(v, f"the {side} of {name!r}"))
+                    raise ValueError(f"{what}: constraint {name!r}: side must be 'min' or 'max', not {side!r}")
+                labels = _constraint_rows(m, name, side, what, PICK)[0]
+                set_rhs(by_index[labels[0]], _number(v, f"the {side} of {name!r}", what))
         else:
-            labels = _constraint_rows(m, name, None, WHAT, PICK)[0]
-            v = _number(value, f"the right-hand side of {name!r}")
+            labels = _constraint_rows(m, name, None, what, PICK)[0]
+            v = _number(value, f"the right-hand side of {name!r}", what)
             # one row, or an equality: upper row, then lower row (Equality.setRightHandSide, expressions.ts:240-245)
             for c in sorted((by_index[i] for i in labels), key=lambda c: not c.isUpperBound):
                 set_rhs(c, v)
-    for vid, value in _entries(spec, "cost"):  # Model.setCost (model.ts:247-256): no skip for an unchanged cost
-        var = _free_variable(m, vid, WHAT)
-        v = _number(value, f"the cost of {vid!r}")
+    for vid, value in _entries(spec, "cost", what):  # Model.setCost (model.ts:247-256): no skip for an unchanged cost
+        var = _free_variable(m, vid, what)
+        v = _number(value, f"the cost of {vid!r}", what)
         difference = v - cost.get(var, var.cost)
         if not m.isMinimization:
             difference = -difference

@@ -8,6 +8,7 @@ from . import validation
 from .conflict import Conflict as _conflict
 from .frontier import Frontier as _frontier
 from .lexicographic import Lexicographic as _lexicographic
+from .mip_scenarios import Scenarios as _scenarios
 from .mip_variability import Variability as _variability
 from .model import Model, object_keys
 from .polyopt import Polyopt
@@ -100,6 +101,14 @@ class Solver:
         return _variability(self, model, gap, absolute_gap, variables, constraints, points, max_nodes, width, precision,
                             validate)
 
+    def Scenarios(self, model: dict, cases, *, width=None, precision: Optional[float] = None,
+                  validate: bool = False) -> list:
+        """What-if scenarios of a model: for each case {"rhs": {constraint: value or {"min", "max"}}, "cost": {variable:
+        value}}, exactly Solve() of the model with those values written in and presolve off, every scenario's branch
+        and cut run side by side on the device (mip_scenarios.py, DESIGN.md section 2p).  `width` tunes the batching
+        only."""
+        return _scenarios(self, model, cases, width, precision, validate)
+
     def _instance(self, model: Any, precision: Optional[float]) -> Model:
         if isinstance(model, dict):
             options = model.get("options") or {}
@@ -173,6 +182,10 @@ def Pool(model: dict, k=10, gap=0.0, absolute_gap=0.0, precision: Optional[float
 def Conflict(model: dict, max_nodes=10000, width=None, depth=None, precision: Optional[float] = None,
              validate: bool = False) -> dict:
     return solver.Conflict(model, max_nodes, width, depth, precision, validate)
+
+
+def Scenarios(model: dict, cases, *, width=None, precision: Optional[float] = None, validate: bool = False) -> list:
+    return solver.Scenarios(model, cases, width=width, precision=precision, validate=validate)
 
 
 def Variability(model: dict, gap=0.0, absolute_gap=0.0, variables=None, constraints=None, points=False,

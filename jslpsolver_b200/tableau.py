@@ -553,6 +553,35 @@ class GpuTableau:
         store["result"] = ev.value if is_min else -ev.value
         return store
 
+    def bnb_batch(self, col0, row0, tolerance: float = 0.0, max_nodes: int = 0, width: int = 0,
+                  check_cycles: Optional[bool] = None) -> dict:
+        """jslp_bnb_batch: branch and cut (the default service) of this tableau with rows 1.. of column 0 replaced by
+        col0[s] and row 0 by row0[s], for every scenario s (DESIGN.md section 2p); the root LP alone without integer
+        variables.  Returns the per-scenario BnbStatus list, the final column 0 and row labels (rhs / vrow, n x
+        row_stride, `height` entries each) and the kernel launches of the call.  The tableau, its snapshot and its
+        scalar state are left as they were."""
+        c0 = np.ascontiguousarray(col0, dtype=np.float64)
+        r0 = np.ascontiguousarray(row0, dtype=np.float64)
+        n = c0.shape[0]
+        if n and (c0.shape[1] != self.height or r0.shape != (n, self.width)):
+            raise ValueError(f"bnb_batch: column 0 / row 0 must be n x {self.height} / n x {self.width}")
+        m = self.model
+        opts = BnbOpts()
+        opts.tolerance = float(tolerance)
+        opts.is_minimization = int(bool(getattr(m, "isMinimization", True)))
+        opts.check_cycles = self._check_cycles() if check_cycles is None else int(bool(check_cycles))
+        opts.max_spec_batch = int(width)
+        opts.rank, opts.n_ranks = 0, 1
+        opts.max_nodes = int(max_nodes)
+        stride = self.height + 2 * getattr(self, "nInts", 0)
+        status = (BnbStatus * max(1, n))()
+        rhs, vrow = np.zeros((n, stride), dtype=np.float64), np.zeros((n, stride), dtype=np.int32)
+        height = np.zeros(n, dtype=np.int32)
+        _lib.check(self.context.lib.jslp_bnb_batch(self._h(), c0.ctypes.data, r0.ctypes.data, n, C.byref(opts), stride,
+                                                   status, rhs.ctypes.data, vrow.ctypes.data, height.ctypes.data))
+        return {"status": [status[i] for i in range(n)], "rhs": rhs, "vrow": vrow, "height": height,
+                "launches": int(status[0].kernel_launches) if n else 0}
+
     def node_log(self) -> np.ndarray:
         n = C.c_int64()
         L = self.context.lib
