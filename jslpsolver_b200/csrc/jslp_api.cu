@@ -77,7 +77,6 @@ struct ResidentBufs {
     int4 *d_logs = nullptr, *h_logs = nullptr;      // full logs: device memory, fetched only when needed
     int cap_nodes = 0, cap_cuts = 0;
     size_t cap_log_entries = 0;
-    int smem_set = 0;
     void release() {
         cudaFree(d_logs);
         cudaFreeHost(h_cuts); cudaFreeHost(h_off); cudaFreeHost(h_out); cudaFreeHost(h_logs);
@@ -798,6 +797,8 @@ static void fill_status(jslp_tab *t, jslp_lp_status *o, const Rec &r, int cycled
 }
 
 static size_t node_smem_bytes(int Hcap, int W, int *Ws_out);
+template <int MODE>
+static int batch_launch(jslp_tab *t, const NodeBatchDev &nb, int n, size_t smem, double *rhs, int32_t *vrow);
 static void finish_lp_flags(jslp_tab *t, int only_phase, int cycled, const Rec &last);
 
 // Engine 4: the whole simplex() of a small tableau in ONE launch, tableau resident in shared
@@ -828,14 +829,8 @@ static int run_lp_resident(jslp_tab *t, int check_cycles, jslp_lp_status *out, b
     nb.wb_M = snap.M; nb.wb_vrow = snap.vrow; nb.wb_vcol = snap.vcol;
     nb.H0 = t->H; nb.root_stride = t->stride; nb.first_index = t->lastElementIndex;
     nb.Hcap = t->H; nb.Ws = Ws; nb.log_cap = log_cap; nb.max_pivots = log_cap - 2;
-    if ((int)smem > rb.smem_set) {
-        CK(cudaFuncSetAttribute(k_node_batch<NODE_BRANCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        rb.smem_set = (int)smem;
-    }
-    k_node_batch<NODE_BRANCH><<<1, NODE_THREADS, smem, s>>>(t->d_T, nb);
-    ctx->launches += 1;
-    CK(cudaGetLastError());
-    CK(cudaStreamSynchronize(s));
+    rc = batch_launch<NODE_BRANCH>(t, nb, 1, smem, nullptr, nullptr);
+    if (rc) return rc;
     const NodeResult r = rb.h_out[0].r;
     if (r.overflow || r.log_n > log_cap) return JSLP_OK;
     if (r.log_n <= NODE_LOG_HEAD) {
@@ -844,15 +839,8 @@ static int run_lp_resident(jslp_tab *t, int check_cycles, jslp_lp_status *out, b
         CK(cudaMemcpyAsync(rb.h_logs, rb.d_logs, sizeof(int4) * (size_t)r.log_n, cudaMemcpyDeviceToHost, s));
         CK(cudaStreamSynchronize(s));
     }
-    if (check_cycles) {
-        std::vector<long long> h1, h2;
-        int cs, cl;
-        for (int k = 0; k < r.log_n; k++) {
-            std::vector<long long> &h = ((rb.h_logs[k].x >> 30) & 1) ? h2 : h1;
-            h.push_back(((long long)rb.h_logs[k].z << 32) | (unsigned int)rb.h_logs[k].w);
-            if (cycle_hit(h, &cs, &cl)) return JSLP_OK;  // exact stop-before-repeat semantics: HBM path
-        }
-    }
+    if (check_cycles && first_cycle(rb.h_logs, r.log_n) >= 0)
+        return JSLP_OK;  // exact stop-before-repeat semantics: HBM path
     // adopt the result
     CK(cudaMemcpy2DAsync(t->hd.M, sizeof(double) * t->stride, snap.M, sizeof(double) * t->stride,
                          sizeof(double) * t->W, t->H, cudaMemcpyDeviceToDevice, s));
@@ -1369,6 +1357,7 @@ extern "C" int jslp_pivot_log(jslp_tab *t, int32_t *entries, int cap, int *n) {
 #include "jslp_dynamic.cuh"
 #include "jslp_comm.cuh"
 #include "jslp_bnb_enhanced.cuh"
+#include "jslp_batch.cuh"
 #include "jslp_bnb.cuh"
 #include "jslp_sensitivity.cuh"
 #include "jslp_iis.cuh"

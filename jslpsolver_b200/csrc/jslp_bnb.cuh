@@ -70,6 +70,24 @@ static int eval_node_streaming(jslp_tab *t, const jslp_bnb::Branch &b, int check
     return JSLP_OK;
 }
 
+// A node LP the device ran on its own (node kernel or node slot) as eval_node_streaming reads it from the tableau:
+// the status (ST_OPTIMAL, ST_UNBOUNDED, else infeasible), the raw evaluation, the pivots and the integrality scan,
+// which only a feasible node carries.
+static jslp_bnb::NodeEval node_eval(int status, double eval_raw, int pivots, int is_integral, int branch_var,
+                                    double branch_value, double precision) {
+    jslp_bnb::NodeEval ev;
+    ev.valid = true;
+    ev.pivots = pivots;
+    ev.optimal = status == ST_OPTIMAL;
+    ev.bounded = status != ST_UNBOUNDED;
+    ev.feasible = status == ST_OPTIMAL || status == ST_UNBOUNDED;
+    // infeasible: the evaluation is never read by the commit loop; 0 keeps it rank-independent on the wire
+    ev.evaluation = status == ST_OPTIMAL ? jslp_round_evaluation(eval_raw, precision)
+                                         : (status == ST_UNBOUNDED ? -INFINITY : 0.0);
+    if (ev.feasible) { ev.is_integral = is_integral; ev.branch_var = branch_var; ev.branch_value = branch_value; }
+    return ev;
+}
+
 // ---- K3: HBM-resident node batch (jslp_slots.cuh) ---------------------------------------------
 // Largest number of slots for which every slot still runs the ping-pong step (at most 32 rows per row CTA,
 // all B * (G + 2) CTAs co-resident), capped by the option and by what keeps the buffers being written in L2.
@@ -305,18 +323,9 @@ static int eval_nodes_slots(jslp_tab *t, jslp_bnb::Branch *const *nodes, int n, 
                 }
                 if (hit) { account(i, r.p1 + r.p2); redo.push_back(i); node_of[b] = -1; done++; continue; }
                 if (r.status == ST_RUNNING) continue;
-                jslp_bnb::NodeEval &ev = nodes[i]->ev;
-                ev.valid = true;
-                ev.pivots = r.p1 + r.p2;
-                ev.optimal = r.status == ST_OPTIMAL;
-                ev.bounded = r.status != ST_UNBOUNDED;
-                ev.feasible = r.status == ST_OPTIMAL || r.status == ST_UNBOUNDED;
-                ev.evaluation = r.status == ST_OPTIMAL ? jslp_round_evaluation(r.eval_raw, t->precision)
-                                                       : (r.status == ST_UNBOUNDED ? -INFINITY : 0.0);
                 const MipOut &mo = ns.h_out[b].mip;
-                ev.is_integral = ev.feasible ? mo.is_integral : 0;
-                ev.branch_var = ev.feasible ? mo.var_index : -1;
-                ev.branch_value = ev.feasible ? mo.value : 0.0;
+                const jslp_bnb::NodeEval &ev = nodes[i]->ev =
+                    node_eval(r.status, r.eval_raw, r.p1 + r.p2, mo.is_integral, mo.var_index, mo.value, t->precision);
                 if (ev.feasible && ev.is_integral && ev.evaluation < *U) *U = ev.evaluation;
                 account(i, ev.pivots);
                 if (dbg) fprintf(stderr, "slot node: slot %d cuts %d pivots %d+%d status %d\n", b, (int)nodes[i]->cuts.size(), r.p1, r.p2, r.status);
@@ -342,109 +351,48 @@ static int eval_nodes_slots(jslp_tab *t, jslp_bnb::Branch *const *nodes, int n, 
     return JSLP_OK;
 }
 
-static size_t node_smem_bytes(int Hcap, int W, int *Ws_out) {
-    const int Ws = (W + 1) & ~1;  // even row stride: 16-byte aligned rows (TMA restore)
-    if (Ws_out) *Ws_out = Ws;
-    return sizeof(double) * ((size_t)Hcap * Ws + 2 * (size_t)Ws + Hcap + 1) + sizeof(CutDev) * (size_t)Hcap +
-           sizeof(int) * (2 * (size_t)Hcap + W) + 16;
-}
-
-static bool resident_fits(const jslp_tab *t, int Hcap) {
-    return t->nOpt == 0 && node_smem_bytes(Hcap, t->W, nullptr) <= (size_t)t->ctx->max_smem_optin - 4096;
-}
-
-// Evaluates nodes[0..n) with one CTA each (k_node_batch).  Nodes whose log shows a cycle or that
-// hit the in-kernel pivot cap are re-evaluated on the HBM path (exact cycle semantics there).
+// Evaluates nodes[0..n) with one CTA each (k_node_batch<NODE_BRANCH>).  Nodes whose log shows a cycle or that hit the
+// in-kernel pivot or log cap are re-evaluated on the HBM path (exact cycle semantics there).
 static int eval_nodes_resident(jslp_tab *t, jslp_bnb::Branch *const *nodes, int n, int check_cycles) {
-    jslp_ctx *ctx = t->ctx;
-    cudaStream_t s = ctx->stream;
-    ResidentBufs &rb = t->rbufs;
-    int maxc = 0, totc = 0;
-    for (int i = 0; i < n; i++) {
-        maxc = std::max(maxc, (int)nodes[i]->cuts.size());
-        totc += (int)nodes[i]->cuts.size();
-    }
-    const int Hcap = t->saved.H + maxc;
-    int Ws = 0;
-    const size_t smem = node_smem_bytes(Hcap, t->W, &Ws);
-    const int log_cap = t->node_log_cap;
-    int rc = rb.ensure(n, totc, log_cap);
-    if (rc) return rc;
-    int off = 0;
-    for (int i = 0; i < n; i++) {
-        rb.h_off[i] = off;
-        for (const jslp_cut &c : nodes[i]->cuts) {
-            rb.h_cuts[off].type = c.type; rb.h_cuts[off].var_index = c.var_index; rb.h_cuts[off].value = c.value;
-            off++;
-        }
-    }
-    rb.h_off[n] = off;
+    const ResidentBufs &rb = t->rbufs;
     NodeBatchDev nb;
-    memset(&nb, 0, sizeof(nb));
-    nb.rootM = t->saved.M; nb.root_vrow = t->saved.vrow; nb.root_vcol = t->saved.vcol;
-    nb.cuts = rb.dv_cuts; nb.cut_off = rb.dv_off; nb.out = rb.dv_out; nb.logs = rb.d_logs;
-    nb.H0 = t->saved.H; nb.root_stride = t->stride; nb.first_index = t->saved.lastElementIndex;
-    nb.Hcap = Hcap; nb.Ws = Ws; nb.log_cap = log_cap; nb.max_pivots = 100000;
-    if (n <= NODE_INLINE_OFF) {
-        nb.n_inline = n;
-        for (int i = 0; i <= n; i++) nb.cut_off_inline[i] = rb.h_off[i];
-    }
-    if ((int)smem > rb.smem_set) {
-        CK(cudaFuncSetAttribute(k_node_batch<NODE_BRANCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        rb.smem_set = (int)smem;
-    }
-    k_node_batch<NODE_BRANCH><<<n, NODE_THREADS, smem, s>>>(t->d_T, nb);
-    ctx->launches += 1;
-    CK(cudaGetLastError());
-    CK(cudaStreamSynchronize(s));  // inputs and outputs are mapped host memory: nothing to copy
+    size_t smem = 0;
+    int rc = batch_fill(t, t->saved.M, t->saved.vrow, t->saved.vcol, t->saved.H, t->saved.lastElementIndex, n, nb,
+                        &smem);
+    if (rc) return rc;
+    rc = branch_cuts(t, n, [&](int k) { return nodes[k]; }, nb);
+    if (rc) return rc;
+    int maxc = 0;
+    for (int i = 0; i < n; i++) maxc = std::max(maxc, (int)nodes[i]->cuts.size());
+    nb.Hcap = t->saved.H + maxc;
+    smem = node_smem_bytes(nb.Hcap, t->W, nullptr);
+    rc = batch_launch<NODE_BRANCH>(t, nb, n, smem, nullptr, nullptr);
+    if (rc) return rc;
     long long slowest = 0;
     bool need_full = false;
     static const bool dbg = getenv("JSLP_DEBUG") != nullptr;  // per-node timeline on stderr (scripts/node_timeline.py)
     for (int i = 0; i < n; i++) {
-        if (dbg) {
-            const NodeResult &q = rb.h_out[i].r;
+        const NodeResult &q = rb.h_out[i].r;
+        if (dbg)
             fprintf(stderr, "node r%d n%d i%d cuts %d piv %d+%d: off %lld restore %lld cuts %lld pivots %lld mip %lld end %lld cy %lld %lld %lld %lld %lld %lld\n",
-                    (int)ctx->launches, n, i, (int)nodes[i]->cuts.size(), q.p1, q.p2, q.tl[0], q.tl[1], q.tl[2], q.tl[3], q.tl[4], q.t_ns, q.cy[0], q.cy[1], q.cy[2], q.cy[3], q.cy[4], q.cy[5]);
-        }
-        slowest = std::max(slowest, rb.h_out[i].r.t_ns);
-        if (check_cycles && !rb.h_out[i].r.overflow && rb.h_out[i].r.log_n > NODE_LOG_HEAD) need_full = true;
+                    (int)t->ctx->launches, n, i, (int)nodes[i]->cuts.size(), q.p1, q.p2, q.tl[0], q.tl[1], q.tl[2], q.tl[3], q.tl[4], q.t_ns, q.cy[0], q.cy[1], q.cy[2], q.cy[3], q.cy[4], q.cy[5]);
+        slowest = std::max(slowest, q.t_ns);
+        need_full |= check_cycles && !q.overflow && q.log_n > NODE_LOG_HEAD;
     }
     t->node_kernel_ns += slowest;
-    if (need_full) {  // rare: a node with a long pivot sequence, fetch the complete logs
-        CK(cudaMemcpyAsync(rb.h_logs, rb.d_logs, sizeof(int4) * (size_t)n * log_cap, cudaMemcpyDeviceToHost, s));
-        CK(cudaStreamSynchronize(s));
-    }
-    std::vector<int> redo_list;
+    rc = batch_fetch_logs(t, n, need_full);  // rare: a node with a long pivot sequence
+    if (rc) return rc;
+    std::vector<int> redo;
     for (int i = 0; i < n; i++) {
         const NodeResult &r = rb.h_out[i].r;
-        jslp_bnb::NodeEval &ev = nodes[i]->ev;
-        bool redo = r.overflow != 0;
-        if (!redo && check_cycles) {
-            std::vector<long long> h1, h2;
-            int cs, cl;
-            const int4 *lg = r.log_n > NODE_LOG_HEAD ? rb.h_logs + (size_t)i * log_cap : rb.h_out[i].log_head;
-            for (int k = 0; k < r.log_n && k < log_cap && !redo; k++) {
-                std::vector<long long> &h = ((lg[k].x >> 30) & 1) ? h2 : h1;
-                h.push_back(((long long)lg[k].z << 32) | (unsigned int)lg[k].w);
-                if (cycle_hit(h, &cs, &cl)) redo = true;
-            }
+        if (r.overflow || (check_cycles && first_cycle(batch_log(t, i), std::min(r.log_n, t->node_log_cap)) >= 0)) {
+            redo.push_back(i);  // second pass: the HBM path may reuse rb's buffers
+            continue;
         }
-        if (redo) { redo_list.push_back(i); continue; }  // second pass: the HBM path may reuse rb's buffers
-        ev.valid = true;
-        ev.pivots = r.p1 + r.p2;
-        ev.optimal = r.status == ST_OPTIMAL;
-        ev.bounded = r.status != ST_UNBOUNDED;
-        ev.feasible = r.status == ST_OPTIMAL || r.status == ST_UNBOUNDED;
-        if (r.status == ST_OPTIMAL) {
-            ev.evaluation = jslp_round_evaluation(r.eval_raw, t->precision);
-        } else if (r.status == ST_UNBOUNDED) {
-            ev.evaluation = -INFINITY;
-        } else {
-            ev.evaluation = 0.0;  // infeasible: never read by the commit loop; rank-independent on the wire
-        }
-        ev.is_integral = r.is_integral; ev.branch_var = r.branch_var; ev.branch_value = r.branch_value;
+        nodes[i]->ev =
+            node_eval(r.status, r.eval_raw, r.p1 + r.p2, r.is_integral, r.branch_var, r.branch_value, t->precision);
     }
-    for (int i : redo_list) {
+    for (int i : redo) {
         rc = eval_node_streaming(t, *nodes[i], check_cycles, nodes[i]->ev);
         if (rc) return rc;
     }
@@ -476,7 +424,6 @@ extern "C" int jslp_branch_and_cut(jslp_tab *t, const jslp_bnb_opts *opts, jslp_
     Tree tree(t->nOpt);
     Frontier &branches = tree.branches;
     const int &iterations = tree.iterations;
-    const double &bestEvaluation = tree.bestEvaluation;
     int rounds = 0;
     const int check_cycles = opts->check_cycles;
     bool timed_out = false;
@@ -526,25 +473,7 @@ extern "C" int jslp_branch_and_cut(jslp_tab *t, const jslp_bnb_opts *opts, jslp_
         const int width = iterations == 0 ? 1 : K;  // the root decides everything: alone
         std::vector<Frontier::Entry> taken;
         std::vector<Branch *> todo;
-        // U = incumbent bound of the round (see eval_nodes_slots): committed incumbent and cached integral results
-        double U = bestEvaluation;
-        // the scan is bounded: once the un-evaluated nodes thin out it would otherwise walk the whole heap every
-        // round (entries with a cached result are popped and pushed back); candidates that far down the pop order
-        // are not popped before the next round anyway
-        const size_t scan_cap = (size_t)width * 4 + 32;
-        while (!branches.empty() && (int)todo.size() < width && taken.size() < scan_cap) {
-            Frontier::Entry e = branches.pop_entry();
-            // nodes that will be skipped at pop (branch-and-cut.ts:90-92) stay in the heap -- their pop
-            // still consumes a loop iteration of the reference -- but are never evaluated
-            if (e.b->ev.valid) {
-                if (e.b->ev.feasible && e.b->ev.is_integral && e.b->ev.evaluation < U) U = e.b->ev.evaluation;
-            } else if (!(e.b->relaxedEvaluation > U)) {
-                todo.push_back(e.b.get());
-            } else {
-                pruned++;
-            }
-            taken.push_back(std::move(e));
-        }
+        double U = tree.speculate(width, taken, todo, pruned);  // the round's incumbent bound (see eval_nodes_slots)
         const auto t_eval = now();
         if (!todo.empty()) {
             rounds++;
@@ -591,7 +520,7 @@ extern "C" int jslp_branch_and_cut(jslp_tab *t, const jslp_bnb_opts *opts, jslp_
                     from_wire(todo[i]->ev, &wire[((size_t)(i % n_ranks) * per + i / n_ranks) * WIRE_DOUBLES]);
             }
         }
-        for (auto &e : taken) branches.push_entry(std::move(e));  // original seq: order unchanged
+        tree.put_back(taken);
         if (iterations == 0) root_ms += ms_since(t_eval);
         eval_ms += ms_since(t_eval);
         const auto t_commit = now();
@@ -631,25 +560,22 @@ extern "C" int jslp_branch_and_cut(jslp_tab *t, const jslp_bnb_opts *opts, jslp_
     int n_best = 0;
     int64_t pivots = tree.pivots;
     const std::unique_ptr<Branch> &bestBranch = tree.bestBranch;
-    if (!tree.early_return) {
-        const Branch *fin = bestBranch ? bestBranch.get() : tree.lastCommitted.get();
-        if (fin && (bestBranch || iterations > 1)) {
-            const auto t_fin = now();
-            NodeEval ev;
-            int rc = eval_node_streaming(t, *fin, check_cycles, ev);
-            if (rc) return rc;
-            nodes++;
-            if (bestBranch) {
-                pivots += ev.pivots;
-                if (ev.optimal) t->simplexIters += ev.n_optimal >= 0 ? ev.n_optimal : 1;
-            }
-            final_ms = ms_since(t_fin);
-        }
+    if (const Branch *fin = tree.final_branch()) {
+        const auto t_fin = now();
+        NodeEval ev;
+        int rc = eval_node_streaming(t, *fin, check_cycles, ev);
+        if (rc) return rc;
+        nodes++;
         if (bestBranch) {
-            n_best = (int)bestBranch->cuts.size();
-            if (best_cuts)
-                for (int i = 0; i < n_best && i < best_cuts_cap; i++) best_cuts[i] = bestBranch->cuts[i];
+            pivots += ev.pivots;
+            if (ev.optimal) t->simplexIters += ev.n_optimal >= 0 ? ev.n_optimal : 1;
         }
+        final_ms = ms_since(t_fin);
+    }
+    if (bestBranch && !tree.early_return) {
+        n_best = (int)bestBranch->cuts.size();
+        if (best_cuts)
+            for (int i = 0; i < n_best && i < best_cuts_cap; i++) best_cuts[i] = bestBranch->cuts[i];
     }
     t->bncIterations = iterations;
     t->node_log = std::move(tree.node_log);

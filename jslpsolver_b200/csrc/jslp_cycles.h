@@ -5,25 +5,11 @@
 #include <unordered_map>
 #include <vector>
 
-// checkForCycles (simplex.ts:415-440) under its calling discipline (called after every push,
-// stops at the first hit): a repeated block must end at the newest element, so only suffix
-// squares are examined; the literal scan reports the smallest start = the longest block.
-static bool cycle_hit(const std::vector<long long> &h, int *start, int *len) {
-    const long n = (long)h.size();
-    for (long L = n / 2; L >= 1; L--) {
-        const long e1 = n - 2 * L, e2 = n - L;
-        if (h[e1] != h[e2]) continue;
-        bool eq = true;
-        for (long i = 1; i < L; i++)
-            if (h[e1 + i] != h[e2 + i]) { eq = false; break; }
-        if (eq) { *start = (int)e1; *len = (int)L; return true; }
-    }
-    return false;
-}
-
-// The same test in O(occurrences of the newest pair) per push instead of O(n): a block of length L
-// that repeats up to the newest element needs h[n-1-L] == h[n-1], so only earlier positions of the
-// newest pair are candidate block ends (largest L first, as the literal scan reports it).
+// checkForCycles (simplex.ts:415-440) under its calling discipline (called after every push, stops at the first hit):
+// a repeated block must end at the newest element, so only suffix squares are examined, and the literal scan reports
+// the smallest start = the longest block.  A block of length L that repeats up to the newest element needs
+// h[n-1-L] == h[n-1], so only earlier positions of the newest pair are candidate block ends (largest L first): each
+// push costs O(occurrences of the newest pair) instead of O(n).
 struct CycleHist {
     std::vector<long long> h;
     std::unordered_map<long long, std::vector<int>> pos;
@@ -45,3 +31,15 @@ struct CycleHist {
         return hit;
     }
 };
+
+// The index of the first entry of a node pivot log that closes a repeat, with one (leaving, entering) history per phase
+// (simplex.ts:27,102), or -1.  An entry's .x carries the phase in bit 30, its .z / .w the pair.
+template <typename Entry>
+static int first_cycle(const Entry *lg, int n) {
+    CycleHist h[2];
+    int cs, cl;
+    for (int k = 0; k < n; k++)
+        if (h[(lg[k].x >> 30) & 1].push_and_check(((long long)lg[k].z << 32) | (unsigned int)lg[k].w, &cs, &cl))
+            return k;
+    return -1;
+}

@@ -94,24 +94,18 @@ static int forest_hbm(Forest &f, const ForestNode &n, bool root) {
 static int forest_resident(Forest &f, const ForestNode *nodes, int n, bool root, bool outputs,
                            std::vector<const ForestNode *> &redo) {
     jslp_tab *t = f.t;
-    ResidentBufs &rb = t->rbufs;
-    std::vector<jslp_cut> cuts;
-    std::vector<int32_t> off((size_t)n + 1, 0);
-    std::vector<int> idx((size_t)n), root_of((size_t)n);
+    const ResidentBufs &rb = t->rbufs;
+    std::vector<int> root_of((size_t)n);
     int maxc = 0;
     for (int k = 0; k < n; k++) {
-        const std::vector<jslp_cut> &c = nodes[k].b->cuts;
-        cuts.insert(cuts.end(), c.begin(), c.end());
-        off[k + 1] = (int32_t)cuts.size();
-        idx[k] = k;
         root_of[k] = nodes[k].tree;
-        maxc = std::max(maxc, (int)c.size());
+        maxc = std::max(maxc, (int)nodes[k].b->cuts.size());
     }
     NodeBatchDev nb;
     size_t smem = 0;
     int rc = batch_fill(t, f.baseM, f.base_vrow, f.base_vcol, f.H0, t->saved.lastElementIndex, n, nb, &smem);
     if (rc) return rc;
-    rc = batch_cuts(t, cuts.empty() ? nullptr : cuts.data(), off.data(), idx.data(), n, nb);
+    rc = branch_cuts(t, n, [&](int k) { return nodes[k].b; }, nb);
     if (rc) return rc;
     nb.Hcap = f.H0 + maxc;
     smem = node_smem_bytes(nb.Hcap, t->W, nullptr);
@@ -145,15 +139,8 @@ static int forest_resident(Forest &f, const ForestNode *nodes, int n, bool root,
             redo.push_back(&nodes[k]);
             continue;
         }
-        jslp_bnb::NodeEval &ev = nodes[k].b->ev;  // as eval_nodes_resident reads a node
-        ev.valid = true;
-        ev.pivots = r.p1 + r.p2;
-        ev.optimal = r.status == ST_OPTIMAL;
-        ev.bounded = r.status != ST_UNBOUNDED;
-        ev.feasible = r.status == ST_OPTIMAL || r.status == ST_UNBOUNDED;
-        ev.evaluation = r.status == ST_OPTIMAL ? jslp_round_evaluation(r.eval_raw, t->precision)
-                                               : (r.status == ST_UNBOUNDED ? -INFINITY : 0.0);
-        ev.is_integral = r.is_integral; ev.branch_var = r.branch_var; ev.branch_value = r.branch_value;
+        nodes[k].b->ev = node_eval(r.status, r.eval_raw, r.p1 + r.p2, r.is_integral, r.branch_var, r.branch_value,
+                                   t->precision);
         if (outputs) {
             const int Hn = f.H0 + (int)nodes[k].b->cuts.size();
             memcpy(nodes[k].rhs, rhs.data() + (size_t)k * nb.Hcap, sizeof(double) * (size_t)Hn);
@@ -326,40 +313,25 @@ extern "C" int jslp_bnb_batch(jslp_tab *t, const double *col0, const double *row
                 // speculate: the next K un-evaluated open nodes of every live tree in pop order
                 batch.clear();
                 std::vector<std::vector<Frontier::Entry>> taken((size_t)n);
+                std::vector<Branch *> todo;
                 for (int k = 0; k < n; k++) {
                     if (stop[k]) continue;
-                    Tree &tr = trees[k];
-                    double U = tr.bestEvaluation;
-                    const size_t scan_cap = (size_t)K * 4 + 32;
-                    int todo = 0;
-                    while (!tr.branches.empty() && todo < K && taken[k].size() < scan_cap) {
-                        Frontier::Entry e = tr.branches.pop_entry();
-                        if (e.b->ev.valid) {
-                            if (e.b->ev.feasible && e.b->ev.is_integral && e.b->ev.evaluation < U) U = e.b->ev.evaluation;
-                        } else if (!(e.b->relaxedEvaluation > U)) {
-                            batch.push_back(ForestNode{k, e.b.get(), nullptr, nullptr});
-                            todo++;
-                        } else {
-                            pruned[k]++;
-                        }
-                        taken[k].push_back(std::move(e));
-                    }
-                    if (todo) { rounds[k]++; nodes[k] += todo; }
+                    trees[k].speculate(K, taken[k], todo, pruned[k]);
+                    for (Branch *b : todo) batch.push_back(ForestNode{k, b, nullptr, nullptr});
+                    if (!todo.empty()) { rounds[k]++; nodes[k] += (int64_t)todo.size(); }
                 }
                 if (batch.empty()) break;
                 rc = forest_eval(f, batch, false, false, &launch_ctas);
                 if (rc) return rc;
-                for (int k = 0; k < n; k++)
-                    for (auto &e : taken[k]) trees[k].branches.push_entry(std::move(e));
+                for (int k = 0; k < n; k++) trees[k].put_back(taken[k]);
             }
             // the final tableau: the reference re-solves the winner, or the last evaluated node (branch-and-cut.ts:195-197)
             batch.clear();
             std::vector<NodeEval> keep((size_t)n);
             std::vector<std::unique_ptr<Branch>> fins((size_t)n);
             for (int k = 0; k < n; k++) {
-                Tree &tr = trees[k];
-                const Branch *fin = tr.bestBranch ? tr.bestBranch.get() : tr.lastCommitted.get();
-                if (tr.early_return || !fin || !(tr.bestBranch || tr.iterations > 1)) continue;
+                const Branch *fin = trees[k].final_branch();
+                if (!fin) continue;
                 fins[k].reset(new Branch{fin->relaxedEvaluation, fin->cuts, NodeEval()});
                 batch.push_back(ForestNode{k, fins[k].get(), out_rhs(k), out_vrow(k)});
                 height[g0 + k] = H0 + (int)fin->cuts.size();

@@ -83,7 +83,8 @@ struct NodeLogEntry {
 
 // One tree of the default branch-and-cut service (branch-and-cut.ts:54-199): its frontier, its incumbent and the
 // Tableau scalars the reference's loop reads and writes.  step() is one pass of that loop's body (:76-192) over a node
-// whose LP result is cached in Branch::ev; jslp_branch_and_cut and jslp_bnb_batch both commit through it.
+// whose LP result is cached in Branch::ev; speculate() picks the nodes of a round and final_branch() the node re-solved
+// at the end.  jslp_branch_and_cut and jslp_bnb_batch both run their trees through it.
 struct Tree {
     Frontier branches;
     int iterations = 0;
@@ -132,6 +133,46 @@ struct Tree {
         if (e.b->relaxedEvaluation > bestEvaluation) return NEXT;
         pivots += e.b->ev.pivots;
         return commit(std::move(e.b), r.nOpt);
+    }
+
+    // The nodes of a round: pops open nodes in the order step() will, into taken, until todo holds width nodes
+    // without a cached result or the scan has popped 4 * width + 32 entries.  Returns the round's incumbent bound U,
+    // bestEvaluation lowered by every cached integral result on the way.  A node above U is counted in pruned and
+    // never evaluated: it sorts after the node that set U, so by the time step() pops it bestEvaluation <= U <
+    // relaxedEvaluation and it is skipped (branch-and-cut.ts:90-92).  The scan is bounded because once the
+    // un-evaluated nodes thin out it would otherwise walk the whole heap every round; candidates that far down are not
+    // popped before the next round anyway.
+    double speculate(int width, std::vector<Frontier::Entry> &taken, std::vector<Branch *> &todo, int64_t &pruned) {
+        taken.clear();
+        todo.clear();
+        double U = bestEvaluation;
+        const size_t scan_cap = (size_t)width * 4 + 32;
+        while (!branches.empty() && (int)todo.size() < width && taken.size() < scan_cap) {
+            Frontier::Entry e = branches.pop_entry();
+            if (e.b->ev.valid) {
+                if (e.b->ev.feasible && e.b->ev.is_integral && e.b->ev.evaluation < U) U = e.b->ev.evaluation;
+            } else if (!(e.b->relaxedEvaluation > U)) {
+                todo.push_back(e.b.get());
+            } else {
+                pruned++;
+            }
+            taken.push_back(std::move(e));
+        }
+        return U;
+    }
+    // The entries speculate() took back into the frontier, with their original sequence numbers: the pop order is as
+    // it was.
+    void put_back(std::vector<Frontier::Entry> &taken) {
+        for (Frontier::Entry &e : taken) branches.push_entry(std::move(e));
+        taken.clear();
+    }
+
+    // The node the reference re-solves once the loop ends (branch-and-cut.ts:195-197): the incumbent, else the last
+    // committed node when more than one was committed; null after the early return at an integral root.
+    const Branch *final_branch() const {
+        if (early_return) return nullptr;
+        if (bestBranch) return bestBranch.get();
+        return iterations > 1 ? lastCommitted.get() : nullptr;
     }
 
   private:

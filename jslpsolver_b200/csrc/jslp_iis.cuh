@@ -1,5 +1,5 @@
-// jslpsolver_b200/csrc/jslp_iis.cuh -- the scaffolding of the analysis batches and the row-subset batch behind
-// jslp_feasibility_batch and jslp_conflict_batch (included by jslp_api.cu after jslp_bnb.cuh).  No reference
+// jslpsolver_b200/csrc/jslp_iis.cuh -- the row-subset batch behind jslp_feasibility_batch and jslp_conflict_batch
+// (included by jslp_api.cu after jslp_bnb.cuh; its launch helpers are jslp_batch.cuh's).  No reference
 // counterpart: the feasibility test is the one behind Solution.iis() (DESIGN.md 2c), the conflict nodes the ones behind
 // Conflict() (DESIGN.md 2n).
 //
@@ -36,158 +36,6 @@ __global__ void __launch_bounds__(256) k_mip_scan_masked(const TabDev *Tp, MipOu
 }
 
 }  // namespace jslp
-
-// ---- scaffolding of the analysis batches (jslp_feasibility_batch, jslp_conflict_batch, jslp_scenario_batch,
-// jslp_column_batch, jslp_pool_batch) ----------------------------------------------------------------------------------
-
-// One grow-only device block per tab for the per-call inputs and outputs of those batches; none of them holds it
-// across a call of another.
-static int batch_scratch(jslp_tab *t, size_t bytes) {
-    if (bytes <= t->scratch_bytes) return JSLP_OK;
-    cudaFree(t->d_scratch);
-    t->d_scratch = nullptr;
-    t->scratch_bytes = 0;
-    CK(cudaMalloc(&t->d_scratch, bytes));
-    t->scratch_bytes = bytes;
-    return JSLP_OK;
-}
-
-// The scalar Tableau state and the executed-pivot log describe the caller's tableau, not a batch's sets: captured on
-// entry, put back by restore() once the device tableau is restored.
-struct CallerState {
-    int feasible, bounded, iters, unb;
-    double evaluation, best;
-    size_t log_size;
-    explicit CallerState(const jslp_tab *t)
-        : feasible(t->feasible), bounded(t->bounded), iters(t->simplexIters), unb(t->unboundedVar),
-          evaluation(t->evaluation), best(t->bestPossibleEval), log_size(t->host_log.size()) {}
-    void restore(jslp_tab *t) const {
-        t->feasible = feasible; t->bounded = bounded; t->simplexIters = iters; t->unboundedVar = unb;
-        t->evaluation = evaluation; t->bestPossibleEval = best;
-        if (t->host_log.size() > log_size) t->host_log.resize(log_size);
-    }
-};
-
-// The shared-memory node kernel takes a batch of H-row tableaux unless the engine is pinned to 1 or 2; every other
-// set runs on the single-tableau path.
-static bool batch_resident(const jslp_tab *t, int H) { return t->engine != 1 && t->engine != 2 && resident_fits(t, H); }
-
-// Sets per launch of H-row tableaux: the per-set outputs on the device stay bounded (about 32 MB).
-static int batch_chunk(int H) {
-    return (int)std::max<size_t>(1, std::min<size_t>(4096, ((size_t)32 << 20) / ((size_t)12 * H)));
-}
-
-// The fields of a k_node_batch launch of n sets that do not depend on the mode: the root tableau (M, vrow, vcol; H0
-// rows at t's stride, labels handed out from first_index), no room for rows beyond H0, and the records and logs of
-// rbufs, sized for n.  *smem = the launch's dynamic shared memory.
-static int batch_fill(jslp_tab *t, const double *M, const int *vrow, const int *vcol, int H0, int first_index, int n,
-                      NodeBatchDev &nb, size_t *smem) {
-    ResidentBufs &rb = t->rbufs;
-    int rc = rb.ensure(n, 0, t->node_log_cap);
-    if (rc) return rc;
-    int Ws = 0;
-    *smem = node_smem_bytes(H0, t->W, &Ws);
-    memset(&nb, 0, sizeof(nb));
-    nb.rootM = M; nb.root_vrow = vrow; nb.root_vcol = vcol;
-    nb.out = rb.dv_out; nb.logs = rb.d_logs;
-    nb.H0 = H0; nb.root_stride = t->stride; nb.first_index = first_index;
-    nb.Hcap = H0; nb.Ws = Ws; nb.log_cap = t->node_log_cap; nb.max_pivots = 100000;
-    return JSLP_OK;
-}
-
-// The cut rows of sets idx[0..n) to rbufs, where nb reads them: set k's are cuts[cut_off[idx[k]] .. cut_off[idx[k] + 1])
-// (none when cuts is null), in mapped host memory as branch-and-cut's node launches read them, with the offsets inline
-// in nb as well when they fit.
-static int batch_cuts(jslp_tab *t, const jslp_cut *cuts, const int32_t *cut_off, const int *idx, int n,
-                      NodeBatchDev &nb) {
-    ResidentBufs &rb = t->rbufs;
-    int totc = 0;
-    for (int k = 0; cuts && k < n; k++) totc += cut_off[idx[k] + 1] - cut_off[idx[k]];
-    int rc = rb.ensure(n, totc, t->node_log_cap);
-    if (rc) return rc;
-    int c = 0;
-    for (int k = 0; k < n; k++) {
-        rb.h_off[k] = c;
-        for (int h = cuts ? cut_off[idx[k]] : 0, e = cuts ? cut_off[idx[k] + 1] : 0; h < e; h++, c++) {
-            rb.h_cuts[c].type = cuts[h].type; rb.h_cuts[c].var_index = cuts[h].var_index; rb.h_cuts[c].value = cuts[h].value;
-        }
-    }
-    rb.h_off[n] = c;
-    nb.cuts = rb.dv_cuts; nb.cut_off = rb.dv_off;
-    if (n <= NODE_INLINE_OFF) {
-        nb.n_inline = n;
-        for (int k = 0; k <= n; k++) nb.cut_off_inline[k] = rb.h_off[k];
-    }
-    return JSLP_OK;
-}
-
-// The bit-packed masks of n sets: bits[k * words + (j >> 5)] bit (j & 31) = bytes[i * len + j] != 0, with i = idx[k]
-// (i = k when idx is null).
-static std::vector<uint32_t> pack_bits(const uint8_t *bytes, int len, const int *idx, int n, int words) {
-    std::vector<uint32_t> bits((size_t)std::max(1, n * words), 0u);
-    for (int k = 0; k < n; k++) {
-        const uint8_t *b = bytes + (size_t)(idx ? idx[k] : k) * len;
-        for (int j = 0; j < len; j++)
-            if (b[j]) bits[(size_t)k * words + (j >> 5)] |= 1u << (j & 31);
-    }
-    return bits;
-}
-
-// One k_node_batch<MODE> launch of n sets; with out_rhs set, the final columns and labels to rhs / vrow (n x Hcap).
-template <int MODE>
-static int batch_launch(jslp_tab *t, const NodeBatchDev &nb, int n, size_t smem, double *rhs, int32_t *vrow) {
-    jslp_ctx *ctx = t->ctx;
-    cudaStream_t s = ctx->stream;
-    CK(cudaFuncSetAttribute(k_node_batch<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k_node_batch<MODE><<<n, NODE_THREADS, smem, s>>>(t->d_T, nb);
-    ctx->launches += 1;
-    CK(cudaGetLastError());
-    if (nb.out_rhs) {
-        CK(cudaMemcpyAsync(rhs, nb.out_rhs, sizeof(double) * (size_t)n * nb.Hcap, cudaMemcpyDeviceToHost, s));
-        CK(cudaMemcpyAsync(vrow, nb.out_vrow, sizeof(int) * (size_t)n * nb.Hcap, cudaMemcpyDeviceToHost, s));
-    }
-    CK(cudaStreamSynchronize(s));
-    return JSLP_OK;
-}
-
-// The full logs of the last launch's n sets to the host, when need says a set whose log the caller reads outgrew the
-// inline head.
-static int batch_fetch_logs(jslp_tab *t, int n, bool need) {
-    if (!need) return JSLP_OK;
-    cudaStream_t s = t->ctx->stream;
-    ResidentBufs &rb = t->rbufs;
-    CK(cudaMemcpyAsync(rb.h_logs, rb.d_logs, sizeof(int4) * (size_t)n * t->node_log_cap, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    return JSLP_OK;
-}
-
-// Set i's pivot log: the inline head, or the full log batch_fetch_logs brought over; min(log_n, node_log_cap) entries.
-static const int4 *batch_log(const jslp_tab *t, int i) {
-    const NodeOut &o = t->rbufs.h_out[i];
-    return o.r.log_n > NODE_LOG_HEAD ? t->rbufs.h_logs + (size_t)i * t->node_log_cap : o.log_head;
-}
-
-// The index of the first entry of a node log that closes a repeat, with one (leaving, entering) history per phase
-// (simplex.ts:27,102), or -1.
-static int first_cycle(const int4 *lg, int n) {
-    CycleHist h[2];
-    int cs, cl;
-    for (int k = 0; k < n; k++)
-        if (h[(lg[k].x >> 30) & 1].push_and_check(((long long)lg[k].z << 32) | (unsigned int)lg[k].w, &cs, &cl))
-            return k;
-    return -1;
-}
-
-// Column col of the current buffer to out and, with vrow set, the row labels (H entries each).  The host mirror's M
-// is the device's current buffer between calls (run_lp adopts it after every solve).
-static int read_column(jslp_tab *t, int col, double *out, int32_t *vrow) {
-    cudaStream_t s = t->ctx->stream;
-    CK(cudaMemcpy2DAsync(out, sizeof(double), t->hd.M + col, sizeof(double) * t->stride, sizeof(double), t->H,
-                         cudaMemcpyDeviceToHost, s));
-    if (vrow) CK(cudaMemcpyAsync(vrow, t->hd.vrow, sizeof(int) * (size_t)t->H, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    return JSLP_OK;
-}
 
 // ---- row-subset batches (jslp_feasibility_batch, jslp_conflict_batch) ------------------------------------------------
 

@@ -277,3 +277,45 @@ def test_mir_cut_rows_past_256():
     g.simplex()
     assert_lp_parity(g, o, "after MIR cut rows")
     g.close()
+
+
+# ------------------------------------------------------------------ the node kernel's shared-memory limit
+def test_node_kernel_limit_is_shared_by_tabs_of_different_heights():
+    """The dynamic shared-memory limit of k_node_batch belongs to the kernel on the device, not to a tab: a resident LP
+    (engine 4) on a short tab between two branch and cuts of a tall tab on the same context leaves the second branch and
+    cut equal to the first, node log and final column bit for bit."""
+    import ctypes as C
+    from jslpsolver_b200 import _lib, problems
+    from jslpsolver_b200.model import Model
+    from jslpsolver_b200.tableau import GpuTableau
+    model = Model().loadJson(dict(problems.knapsack_mip_model(40, 100, seed=21), options={"presolve": False}))
+    it = model.initial_tableau()
+    assert it.matrix.shape == (141, 41) and not np.any(it.unrestricted)  # node CTAs above 48 KB of shared memory
+    tall = GpuTableau(model.precision)
+    tall.setModel(model)
+    ints = np.ascontiguousarray(it.integerIndices, dtype=np.int32)
+
+    def branch_and_cut():
+        # the same jslp_tab back at the initial tableau: restore() brings back the root's height, the upload its content
+        tall.restore()
+        M, vrow, vcol = (np.ascontiguousarray(a, dtype=d) for a, d in
+                         ((it.matrix, np.float64), (it.varIndexByRow, np.int32), (it.varIndexByCol, np.int32)))
+        _lib.check(tall.context.lib.jslp_tab_upload(tall._h(), M.ctypes.data, vrow.ctypes.data, vcol.ctypes.data, None,
+                                                    M.shape[0] + M.shape[1] - 2, ints.ctypes.data, len(ints), 0, None))
+        tall.branchAndCut()
+        st = tall.lastBnbStatus
+        assert st.node_kernel_ms > 0  # rounds ran in the node kernel
+        counters = tuple(getattr(st, f) for f in ("feasible", "bounded", "is_integral", "iterations", "n_best_cuts",
+                                                   "rounds", "nodes_evaluated", "pivots", "kernel_launches"))
+        return counters, np.float64(st.evaluation).tobytes(), tall.node_log().tobytes(), tall.rhs_column().tobytes()
+
+    first = branch_and_cut()
+    short = GpuTableau(1e-8, context=tall.context)
+    lp = problems.dense_packing_lp_tableau(8, 6, seed=5)
+    short.upload(lp.matrix, lp.varIndexByRow, lp.varIndexByCol)
+    short.set_option(_lib.OPT_ENGINE, _lib.ENGINE_RESIDENT)
+    short.simplex()
+    assert short.lastStatus.engine == _lib.ENGINE_RESIDENT
+    assert branch_and_cut() == first
+    short.close()
+    tall.close()

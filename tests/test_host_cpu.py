@@ -134,9 +134,10 @@ def test_frontier_heap_follows_the_reference_min_heap(tmp_path):
     assert out.returncode == 0 and "FRONTIER OK" in out.stdout, out.stdout + out.stderr
 
 
-def test_cycle_detectors_follow_the_reference_scan(tmp_path):
-    """tests/cpp/cycles_test.cpp: the product's two host-side detectors (jslp_cycles.h) report exactly what a literal
-    restatement of checkForCycles (simplex.ts:415-440) reports, push by push, on 4000 random pivot histories."""
+def test_cycle_history_and_node_log_screen_follow_the_reference_scan(tmp_path):
+    """tests/cpp/cycles_test.cpp: the product's host-side cycle detection (jslp_cycles.h) reports exactly what a literal
+    restatement of checkForCycles (simplex.ts:415-440) reports: CycleHist push by push on 4000 random pivot histories,
+    and first_cycle on 4000 node logs that interleave two phase histories, against the literal scan per phase."""
     import subprocess
     exe = tmp_path / "cycles_test"
     subprocess.run(["g++", "-std=c++17", "-O2", "-Wall", "-I", os.path.join(ROOT, "jslpsolver_b200", "csrc"),

@@ -226,16 +226,16 @@ def test_restatement_matches_highs_on_infeasible_and_unbounded_cases():
 
 
 # ---- the shared commit rule against the oracle's branch and cut --------------------------------------------------------
-def replay_tree(exe, jm: dict):
-    """(node log, iterations, best cut count) of jslp_bnb::Tree over jm (presolve off), every node evaluated by the oracle in the
-    reference's own order (one node at a time: restore the root snapshot, append the cuts, simplex)."""
+def replay_tree(exe, jm: dict, width: int = 1):
+    """(node log, iterations, best cut count) of jslp_bnb::Tree over jm (presolve off), speculating `width` nodes a round
+    after the root, every node evaluated by the oracle from the root snapshot (restore it, append the cuts, simplex)."""
     from oracle import ref_model as R
     model = R.RefModel().loadJson(jm)
     M, vrow, vcol, _, rc = model.build_tableau()
     tab = R.OracleTableau(M, vrow, vcol, precision=model.precision, integers=[v.index for v in model.integerVariables],
                           check_cycles=model.checkForCycles, is_min=model.isMinimization)
     p = subprocess.Popen([str(exe)], stdin=subprocess.PIPE, stdout=subprocess.PIPE, text=True)
-    p.stdin.write(f"{float(model.tolerance or 0)!r} {int(model.isMinimization)} 0\n")
+    p.stdin.write(f"{float(model.tolerance or 0)!r} {int(model.isMinimization)} 0 {width}\n")
     p.stdin.flush()
     while True:
         line = p.stdout.readline().split()
@@ -271,6 +271,7 @@ def tree_exe(tmp_path_factory):
 
 
 def test_commit_rule_reproduces_the_oracle_node_log(tree_exe):
+    """At every speculation width the commits, and so the node log, are the oracle's bit for bit."""
     from conftest import load_bundle
     from oracle import ref_model as R
     b = load_bundle()
@@ -281,10 +282,11 @@ def test_commit_rule_reproduces_the_oracle_node_log(tree_exe):
     for jm in models:
         for spec in [{}] + seeded_cases(jm, 2, seed=9):
             ed = MS.edited(jm, SO.base_model(jm), spec)
-            log, it, nbest = replay_tree(tree_exe, ed)
             sol = R.solve_full(ed, node_log=1 << 16)
             want = sol.tableau.node_log()
-            assert it == sol.iter, (jm.get("name"), spec)
-            assert log.shape == want.shape and np.array_equal(log.view(np.uint64), want.view(np.uint64)), \
-                (jm.get("name"), spec)
-            assert nbest == len(sol.tableau.best_cuts()) or not sol.state.isIntegral
+            for width in (1, 2, 16):
+                log, it, nbest = replay_tree(tree_exe, ed, width)
+                assert it == sol.iter, (jm.get("name"), spec, width)
+                assert log.shape == want.shape and np.array_equal(log.view(np.uint64), want.view(np.uint64)), \
+                    (jm.get("name"), spec, width)
+                assert nbest == len(sol.tableau.best_cuts()) or not sol.state.isIntegral
