@@ -2,7 +2,8 @@
 // (jslp_bnb.cuh, jslp_forest.cuh) and the analysis batches (jslp_feasibility_batch, jslp_conflict_batch,
 // jslp_scenario_batch, jslp_column_batch, jslp_pool_batch, jslp_target_batch).  Included by jslp_api.cu just before
 // jslp_bnb.cuh.  Each caller keeps its own flow, its own single-tableau path and its own verdicts; what is here is the
-// shared-memory budget of a node, the staging of a launch's inputs, the launch itself and the reading of its logs.
+// shared-memory budget of a node, the argument checks and scratch layout of a batch, the route-and-redo order of its
+// sets, the staging of a launch's inputs, the launch itself and the cycle screen of its logs.
 #pragma once
 
 #include <map>
@@ -31,6 +32,17 @@ static int batch_scratch(jslp_tab *t, size_t bytes) {
     return JSLP_OK;
 }
 
+// The parts of one call's scratch block, each at a 16-byte-aligned offset: take() returns the next part's offset, and
+// bytes is what batch_scratch must hold once every part is taken.
+struct ScratchLayout {
+    size_t bytes = 0;
+    size_t take(size_t n) {
+        const size_t at = bytes;
+        bytes += (n + 15) & ~(size_t)15;
+        return at;
+    }
+};
+
 // The scalar Tableau state and the executed-pivot log describe the caller's tableau, not a batch's sets: captured on
 // entry, put back by restore() once the device tableau is restored.
 struct CallerState {
@@ -47,6 +59,18 @@ struct CallerState {
     }
 };
 
+// The offset arrays of a batch of n sets, set i's entries being [off[i], off[i + 1]) of each: every array starts at 0
+// (`first` names that entry in the message) and never decreases.
+static int batch_check_offsets(std::initializer_list<const int32_t *> offsets, int n, const std::string &what,
+                               const char *first = "offsets[0]") {
+    for (const int32_t *off : offsets)
+        if (off[0] != 0) return fail(JSLP_E_INVALID, what + ": " + first + " must be 0");
+    for (int i = 0; i < n; i++)
+        for (const int32_t *off : offsets)
+            if (off[i + 1] < off[i]) return fail(JSLP_E_INVALID, what + ": offsets must not decrease");
+    return JSLP_OK;
+}
+
 // The shared-memory node kernel takes a batch of H-row tableaux unless the engine is pinned to 1 or 2; every other
 // set runs on the single-tableau path.
 static bool batch_resident(const jslp_tab *t, int H) { return t->engine != 1 && t->engine != 2 && resident_fits(t, H); }
@@ -54,6 +78,31 @@ static bool batch_resident(const jslp_tab *t, int H) { return t->engine != 1 && 
 // Sets per launch of H-row tableaux: the per-set outputs on the device stay bounded (about 32 MB).
 static int batch_chunk(int H) {
     return (int)std::max<size_t>(1, std::min<size_t>(4096, ((size_t)32 << 20) / ((size_t)12 * H)));
+}
+
+// The path of each of n sets and the order they run in: set i goes to the node kernel when batch_resident(t,
+// height_of(i)), in launches resident(idx, m, redo) of at most batch_chunk(tallest resident height) sets, or of every
+// resident set at once when !chunked; single(i) then runs the others one after another, the too-tall sets in index
+// order, then the ones the launches put in redo, in launch order.
+template <typename HeightOf, typename Resident, typename Single>
+static int batch_route(const jslp_tab *t, int n, HeightOf height_of, bool chunked, Resident resident, Single single) {
+    std::vector<int> res, redo;
+    int hmax = 1;
+    for (int i = 0; i < n; i++) {
+        const int h = height_of(i);
+        if (batch_resident(t, h)) { res.push_back(i); hmax = std::max(hmax, h); }
+        else redo.push_back(i);
+    }
+    const size_t chunk = chunked ? (size_t)batch_chunk(hmax) : std::max<size_t>(1, res.size());
+    for (size_t k0 = 0; k0 < res.size(); k0 += chunk) {
+        const int rc = resident(res.data() + k0, (int)std::min(chunk, res.size() - k0), redo);
+        if (rc) return rc;
+    }
+    for (const int i : redo) {
+        const int rc = single(i);
+        if (rc) return rc;
+    }
+    return JSLP_OK;
 }
 
 // The fields of a k_node_batch launch of n sets that do not depend on the mode: the root tableau (M, vrow, vcol; H0
@@ -159,21 +208,28 @@ static int batch_launch(jslp_tab *t, const NodeBatchDev &nb, int n, size_t smem,
     return JSLP_OK;
 }
 
-// The full logs of the last launch's n sets to the host, when need says a set whose log the caller reads outgrew the
-// inline head.
-static int batch_fetch_logs(jslp_tab *t, int n, bool need) {
-    if (!need) return JSLP_OK;
-    cudaStream_t s = t->ctx->stream;
-    ResidentBufs &rb = t->rbufs;
-    CK(cudaMemcpyAsync(rb.h_logs, rb.d_logs, sizeof(int4) * (size_t)n * t->node_log_cap, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    return JSLP_OK;
-}
-
-// Set i's pivot log: the inline head, or the full log batch_fetch_logs brought over; min(log_n, node_log_cap) entries.
+// Set i's pivot log: the inline head, or the full log batch_screen brought over; min(log_n, node_log_cap) entries.
 static const int4 *batch_log(const jslp_tab *t, int i) {
     const NodeOut &o = t->rbufs.h_out[i];
     return o.r.log_n > NODE_LOG_HEAD ? t->rbufs.h_logs + (size_t)i * t->node_log_cap : o.log_head;
+}
+
+// The cycle screen of the last launch's n sets: hit[k] = first_cycle of set k's log (per-phase histories) when
+// screened(k), else -1.  The full logs come to the host only when a screened set's log outgrew the inline head.
+template <typename Screened>
+static int batch_screen(jslp_tab *t, int n, Screened screened, std::vector<int> &hit) {
+    const ResidentBufs &rb = t->rbufs;
+    bool need_full = false;
+    for (int k = 0; k < n; k++) need_full |= screened(k) && rb.h_out[k].r.log_n > NODE_LOG_HEAD;
+    if (need_full) {  // rare: a set with a long pivot sequence
+        CK(cudaMemcpyAsync(rb.h_logs, rb.d_logs, sizeof(int4) * (size_t)n * t->node_log_cap, cudaMemcpyDeviceToHost,
+                           t->ctx->stream));
+        CK(cudaStreamSynchronize(t->ctx->stream));
+    }
+    hit.assign((size_t)n, -1);
+    for (int k = 0; k < n; k++)
+        if (screened(k)) hit[k] = first_cycle(batch_log(t, k), std::min(rb.h_out[k].r.log_n, t->node_log_cap));
+    return JSLP_OK;
 }
 
 // Column col of the current buffer to out and, with vrow set, the row labels (H entries each).  The host mirror's M

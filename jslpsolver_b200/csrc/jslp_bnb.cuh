@@ -369,7 +369,6 @@ static int eval_nodes_resident(jslp_tab *t, jslp_bnb::Branch *const *nodes, int 
     rc = batch_launch<NODE_BRANCH>(t, nb, n, smem, nullptr, nullptr);
     if (rc) return rc;
     long long slowest = 0;
-    bool need_full = false;
     static const bool dbg = getenv("JSLP_DEBUG") != nullptr;  // per-node timeline on stderr (scripts/node_timeline.py)
     for (int i = 0; i < n; i++) {
         const NodeResult &q = rb.h_out[i].r;
@@ -377,15 +376,14 @@ static int eval_nodes_resident(jslp_tab *t, jslp_bnb::Branch *const *nodes, int 
             fprintf(stderr, "node r%d n%d i%d cuts %d piv %d+%d: off %lld restore %lld cuts %lld pivots %lld mip %lld end %lld cy %lld %lld %lld %lld %lld %lld\n",
                     (int)t->ctx->launches, n, i, (int)nodes[i]->cuts.size(), q.p1, q.p2, q.tl[0], q.tl[1], q.tl[2], q.tl[3], q.tl[4], q.t_ns, q.cy[0], q.cy[1], q.cy[2], q.cy[3], q.cy[4], q.cy[5]);
         slowest = std::max(slowest, q.t_ns);
-        need_full |= check_cycles && !q.overflow && q.log_n > NODE_LOG_HEAD;
     }
     t->node_kernel_ns += slowest;
-    rc = batch_fetch_logs(t, n, need_full);  // rare: a node with a long pivot sequence
+    std::vector<int> hit, redo;
+    rc = batch_screen(t, n, [&](int i) { return check_cycles && !rb.h_out[i].r.overflow; }, hit);
     if (rc) return rc;
-    std::vector<int> redo;
     for (int i = 0; i < n; i++) {
         const NodeResult &r = rb.h_out[i].r;
-        if (r.overflow || (check_cycles && first_cycle(batch_log(t, i), std::min(r.log_n, t->node_log_cap)) >= 0)) {
+        if (r.overflow || hit[i] >= 0) {
             redo.push_back(i);  // second pass: the HBM path may reuse rb's buffers
             continue;
         }

@@ -100,25 +100,24 @@ static int column_resident(jslp_tab *t, const uint32_t *bits, int words, int s0,
     rc = batch_cuts(t, nullptr, nullptr, nullptr, n, nb);  // no cut rows
     if (rc) return rc;
     // one device block per chunk: masks, final columns, final labels
-    const size_t b_rhs = (sizeof(uint32_t) * (size_t)n * words + 15) & ~(size_t)15;
-    const size_t b_vrow = b_rhs + sizeof(double) * (size_t)n * H0;
-    rc = batch_scratch(t, b_vrow + sizeof(int) * (size_t)n * H0);
+    ScratchLayout L;
+    const size_t b_keep = L.take(sizeof(uint32_t) * (size_t)n * words), b_rhs = L.take(sizeof(double) * (size_t)n * H0);
+    const size_t b_vrow = L.take(sizeof(int) * (size_t)n * H0);
+    rc = batch_scratch(t, L.bytes);
     if (rc) return rc;
     char *base = (char *)t->d_scratch;
-    CK(cudaMemcpyAsync(base, bits + (size_t)s0 * words, sizeof(uint32_t) * (size_t)n * words, cudaMemcpyHostToDevice,
-                       t->ctx->stream));
-    nb.keep = (const uint32_t *)base; nb.keep_words = words;
+    CK(cudaMemcpyAsync(base + b_keep, bits + (size_t)s0 * words, sizeof(uint32_t) * (size_t)n * words,
+                       cudaMemcpyHostToDevice, t->ctx->stream));
+    nb.keep = (const uint32_t *)(base + b_keep); nb.keep_words = words;
     nb.out_rhs = (double *)(base + b_rhs); nb.out_vrow = (int *)(base + b_vrow);
     rc = batch_launch<NODE_COLUMNS>(t, nb, n, smem, rhs + (size_t)s0 * H0, vrow + (size_t)s0 * H0);
     if (rc) return rc;
-    bool need_full = false;
-    for (int i = 0; i < n; i++) need_full |= !rb.h_out[i].r.overflow && rb.h_out[i].r.log_n > NODE_LOG_HEAD;
-    rc = batch_fetch_logs(t, n, need_full);
+    std::vector<int> hit;
+    rc = batch_screen(t, n, [&](int i) { return !rb.h_out[i].r.overflow; }, hit);
     if (rc) return rc;
     for (int i = 0; i < n; i++) {
         const NodeResult &r = rb.h_out[i].r;
-        const bool again = r.overflow || first_cycle(batch_log(t, i), std::min(r.log_n, t->node_log_cap)) >= 0;
-        if (again) { redo.push_back(s0 + i); continue; }
+        if (r.overflow || hit[i] >= 0) { redo.push_back(s0 + i); continue; }
         status[s0 + i] = r.status == ST_OPTIMAL ? COL_OPTIMAL : r.status == ST_UNBOUNDED ? COL_UNBOUNDED : COL_INFEASIBLE;
         eval_raw[s0 + i] = r.eval_raw;
         pivots[s0 + i] = r.p1 + r.p2;
@@ -141,21 +140,16 @@ extern "C" int jslp_column_batch(jslp_tab *t, const uint8_t *keep_cols, int n_se
     std::vector<uint32_t> bits = pack_bits(keep_cols, W, nullptr, n_sets, words);
     for (int i = 0; i < n_sets; i++) bits[(size_t)i * words] |= 1u;
     const CallerState caller(t);
-    std::vector<int> redo;
-    int rc = JSLP_OK;
-    if (batch_resident(t, H0)) {
-        const int chunk = batch_chunk(H0);
-        for (int s0 = 0; s0 < n_sets && rc == JSLP_OK; s0 += chunk)
-            rc = column_resident(t, bits.data(), words, s0, std::min(chunk, n_sets - s0), status, eval_raw, pivots, rhs,
-                                 vrow, redo);
-    } else {
-        for (int i = 0; i < n_sets; i++) redo.push_back(i);
-    }
-    for (size_t k = 0; k < redo.size() && rc == JSLP_OK; k++) {
-        const int i = redo[k];
-        rc = column_hbm(t, bits.data() + (size_t)i * words, words, status + i, eval_raw + i, pivots + i,
-                        rhs + (size_t)i * H0, vrow + (size_t)i * H0);
-    }
+    // every set has the snapshot's height, so either all of them are resident or none, and a launch's are consecutive
+    int rc = batch_route(
+        t, n_sets, [&](int) { return H0; }, true,
+        [&](const int *idx, int m, std::vector<int> &redo) {
+            return column_resident(t, bits.data(), words, idx[0], m, status, eval_raw, pivots, rhs, vrow, redo);
+        },
+        [&](int i) {
+            return column_hbm(t, bits.data() + (size_t)i * words, words, status + i, eval_raw + i, pivots + i,
+                              rhs + (size_t)i * H0, vrow + (size_t)i * H0);
+        });
     const int rc2 = jslp_restore(t);
     if (rc == JSLP_OK) rc = rc2;
     CK(cudaStreamSynchronize(t->ctx->stream));

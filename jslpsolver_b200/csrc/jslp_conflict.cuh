@@ -20,20 +20,19 @@ extern "C" int jslp_conflict_batch(jslp_tab *t, const uint8_t *keep, const uint8
     if (!t->saved.valid) return fail(JSLP_E_INVALID, "conflict_batch needs a snapshot (jslp_save)");
     if (t->nOpt > 0) return fail(JSLP_E_UNSUPPORTED, "conflict_batch: optional objectives are not supported");
     if (n_nodes == 0) return JSLP_OK;
-    if (cut_offsets[0] != 0) return fail(JSLP_E_INVALID, "conflict_batch: cut_offsets[0] must be 0");
+    int rc = batch_check_offsets({cut_offsets}, n_nodes, "conflict_batch", "cut_offsets[0]");
+    if (rc) return rc;
     const int H0 = t->saved.H;
     std::vector<int> height((size_t)n_nodes);  // cost row, kept rows and cut rows of each node
     for (int i = 0; i < n_nodes; i++) {
-        if (cut_offsets[i + 1] < cut_offsets[i]) return fail(JSLP_E_INVALID, "conflict_batch: offsets must not decrease");
         height[i] = kept_height(keep + (size_t)i * H0, H0) + cut_offsets[i + 1] - cut_offsets[i];
         if (height[i] > row_stride)
             return fail(JSLP_E_INVALID, "conflict_batch: row_stride is below a node's height (kept rows plus cuts)");
     }
     const int n_cuts = cut_offsets[n_nodes];
     if (n_cuts > 0 && !cuts) return fail(JSLP_E_INVALID, "conflict_batch: cuts is NULL");
-    for (int k = 0; k < n_cuts; k++)
-        if ((cuts[k].type != 0 && cuts[k].type != 1) || cuts[k].var_index < 0 || cuts[k].var_index >= t->saved.nVars)
-            return fail(JSLP_E_INVALID, "conflict_batch: cut type must be 0 (min) or 1 (max), on a label of the snapshot");
+    rc = pool_check_cuts(t, cuts, n_cuts, "conflict_batch");
+    if (rc) return rc;
     SubsetBatch b;
     b.keep = keep; b.int_keep = int_keep; b.cuts = cuts; b.cut_off = cut_offsets; b.height = height.data();
     b.status = status; b.pivots = pivots; b.is_integral = is_integral; b.branch_var = branch_var;

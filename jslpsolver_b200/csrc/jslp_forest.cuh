@@ -89,36 +89,38 @@ static int forest_hbm(Forest &f, const ForestNode &n, bool root) {
     return JSLP_OK;
 }
 
-// Nodes nodes[0..n) in one k_node_batch<NODE_FOREST> launch (roots when `root`); those whose log shows a cycle or
-// that hit the pivot or log cap go to redo.
-static int forest_resident(Forest &f, const ForestNode *nodes, int n, bool root, bool outputs,
-                           std::vector<const ForestNode *> &redo) {
+// Nodes nodes[idx[0..n)] in one k_node_batch<NODE_FOREST> launch (roots when `root`); those whose log shows a cycle
+// or that hit the pivot or log cap go to redo.
+static int forest_resident(Forest &f, const std::vector<ForestNode> &nodes, const int *idx, int n, bool root,
+                           bool outputs, std::vector<int> &redo) {
     jslp_tab *t = f.t;
     const ResidentBufs &rb = t->rbufs;
+    auto node = [&](int k) -> const ForestNode & { return nodes[idx[k]]; };
     std::vector<int> root_of((size_t)n);
     int maxc = 0;
     for (int k = 0; k < n; k++) {
-        root_of[k] = nodes[k].tree;
-        maxc = std::max(maxc, (int)nodes[k].b->cuts.size());
+        root_of[k] = node(k).tree;
+        maxc = std::max(maxc, (int)node(k).b->cuts.size());
     }
     NodeBatchDev nb;
     size_t smem = 0;
     int rc = batch_fill(t, f.baseM, f.base_vrow, f.base_vcol, f.H0, t->saved.lastElementIndex, n, nb, &smem);
     if (rc) return rc;
-    rc = branch_cuts(t, n, [&](int k) { return nodes[k].b; }, nb);
+    rc = branch_cuts(t, n, [&](int k) { return node(k).b; }, nb);
     if (rc) return rc;
     nb.Hcap = f.H0 + maxc;
     smem = node_smem_bytes(nb.Hcap, t->W, nullptr);
     nb.slot_M = f.slotM; nb.slot_vrow = f.slot_vrow; nb.slot_vcol = f.slot_vcol; nb.slot_pitch = f.pitch;
     if (root) { nb.col0 = f.col0(0); nb.row0 = f.row0(0); }
     // one device block: the slot of each CTA, then the final columns and labels when asked
-    const size_t b_rhs = (sizeof(int) * (size_t)n + 15) & ~(size_t)15;
-    const size_t b_vrow = b_rhs + sizeof(double) * (size_t)n * nb.Hcap;
-    rc = batch_scratch(t, b_vrow + sizeof(int) * (size_t)n * nb.Hcap);
+    ScratchLayout L;
+    const size_t b_root = L.take(sizeof(int) * (size_t)n), b_rhs = L.take(sizeof(double) * (size_t)n * nb.Hcap);
+    const size_t b_vrow = L.take(sizeof(int) * (size_t)n * nb.Hcap);
+    rc = batch_scratch(t, L.bytes);
     if (rc) return rc;
     char *base = (char *)t->d_scratch;
-    CK(cudaMemcpyAsync(base, root_of.data(), sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, t->ctx->stream));
-    nb.root_of = (const int *)base;
+    CK(cudaMemcpyAsync(base + b_root, root_of.data(), sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, t->ctx->stream));
+    nb.root_of = (const int *)(base + b_root);
     std::vector<double> rhs;
     std::vector<int32_t> vrow;
     if (outputs) {
@@ -128,52 +130,33 @@ static int forest_resident(Forest &f, const ForestNode *nodes, int n, bool root,
     }
     rc = batch_launch<NODE_FOREST>(t, nb, n, smem, rhs.data(), vrow.data());
     if (rc) return rc;
-    bool need_full = false;
-    for (int k = 0; k < n; k++)
-        need_full |= f.check_cycles && !rb.h_out[k].r.overflow && rb.h_out[k].r.log_n > NODE_LOG_HEAD;
-    rc = batch_fetch_logs(t, n, need_full);
+    std::vector<int> hit;
+    rc = batch_screen(t, n, [&](int k) { return f.check_cycles && !rb.h_out[k].r.overflow; }, hit);
     if (rc) return rc;
     for (int k = 0; k < n; k++) {
         const NodeResult &r = rb.h_out[k].r;
-        if (r.overflow || (f.check_cycles && first_cycle(batch_log(t, k), std::min(r.log_n, t->node_log_cap)) >= 0)) {
-            redo.push_back(&nodes[k]);
-            continue;
-        }
-        nodes[k].b->ev = node_eval(r.status, r.eval_raw, r.p1 + r.p2, r.is_integral, r.branch_var, r.branch_value,
-                                   t->precision);
+        if (r.overflow || hit[k] >= 0) { redo.push_back(idx[k]); continue; }
+        node(k).b->ev = node_eval(r.status, r.eval_raw, r.p1 + r.p2, r.is_integral, r.branch_var, r.branch_value,
+                                  t->precision);
         if (outputs) {
-            const int Hn = f.H0 + (int)nodes[k].b->cuts.size();
-            memcpy(nodes[k].rhs, rhs.data() + (size_t)k * nb.Hcap, sizeof(double) * (size_t)Hn);
-            memcpy(nodes[k].vrow, vrow.data() + (size_t)k * nb.Hcap, sizeof(int32_t) * (size_t)Hn);
+            const int Hn = f.H0 + (int)node(k).b->cuts.size();
+            memcpy(node(k).rhs, rhs.data() + (size_t)k * nb.Hcap, sizeof(double) * (size_t)Hn);
+            memcpy(node(k).vrow, vrow.data() + (size_t)k * nb.Hcap, sizeof(int32_t) * (size_t)Hn);
         }
     }
     return JSLP_OK;
 }
 
-// Evaluates nodes[0..n) of the current group: resident ones in launches of at most batch_chunk CTAs, then the others
-// and the redone ones on the single-tableau path.  Counts the CTAs of each launch in *ctas.
-static int forest_eval(Forest &f, std::vector<ForestNode> &nodes, bool root, bool outputs, int64_t *ctas) {
-    jslp_tab *t = f.t;
-    std::vector<ForestNode> res;
-    std::vector<const ForestNode *> redo;
-    int maxc = 0;
-    for (const ForestNode &n : nodes) {
-        const int nc = (int)n.b->cuts.size();
-        if (batch_resident(t, f.H0 + nc)) { res.push_back(n); maxc = std::max(maxc, nc); }
-        else redo.push_back(&n);
-    }
-    const int chunk = batch_chunk(f.H0 + maxc);
-    for (size_t k0 = 0; k0 < res.size(); k0 += chunk) {
-        const int m = (int)std::min<size_t>(chunk, res.size() - k0);
-        int rc = forest_resident(f, res.data() + k0, m, root, outputs, redo);
-        if (rc) return rc;
-        *ctas += m;
-    }
-    for (const ForestNode *n : redo) {
-        int rc = forest_hbm(f, *n, root);
-        if (rc) return rc;
-    }
-    return JSLP_OK;
+// Evaluates the nodes of the current group, routed by batch_route on their height (slot rows plus cuts).  Counts the
+// CTAs of each launch in *ctas.
+static int forest_eval(Forest &f, const std::vector<ForestNode> &nodes, bool root, bool outputs, int64_t *ctas) {
+    return batch_route(
+        f.t, (int)nodes.size(), [&](int i) { return f.H0 + (int)nodes[i].b->cuts.size(); }, true,
+        [&](const int *idx, int m, std::vector<int> &redo) {
+            *ctas += m;
+            return forest_resident(f, nodes, idx, m, root, outputs, redo);
+        },
+        [&](int i) { return forest_hbm(f, nodes[i], root); });
 }
 
 extern "C" int jslp_bnb_batch(jslp_tab *t, const double *col0, const double *row0, int n_scenarios,

@@ -88,11 +88,12 @@ static int subset_hbm(jslp_tab *t, const SubsetBatch &b, int i) {
     const int n = (int)rows.size();
     const std::vector<uint32_t> imask =
         b.int_keep ? pack_bits(b.int_keep, t->n_int, &i, 1, (t->n_int + 31) / 32) : std::vector<uint32_t>();
-    const size_t b_mask = (sizeof(int) * (size_t)n + 15) & ~(size_t)15;
-    int rc = batch_scratch(t, b_mask + sizeof(uint32_t) * imask.size());
+    ScratchLayout L;
+    const size_t b_rows = L.take(sizeof(int) * (size_t)n), b_mask = L.take(sizeof(uint32_t) * imask.size());
+    int rc = batch_scratch(t, L.bytes);
     if (rc) return rc;
     cudaStream_t s = t->ctx->stream;
-    int *d_rows = (int *)t->d_scratch;
+    int *d_rows = (int *)((char *)t->d_scratch + b_rows);
     uint32_t *d_mask = (uint32_t *)((char *)t->d_scratch + b_mask);
     CK(cudaMemcpyAsync(d_rows, rows.data(), sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, s));
     if (!imask.empty())
@@ -154,15 +155,15 @@ static int subset_resident(jslp_tab *t, const SubsetBatch &b, const int *idx, in
     const std::vector<uint32_t> kbits = pack_bits(b.keep, H0, idx, n, kw);
     const std::vector<uint32_t> ibits = b.int_keep ? pack_bits(b.int_keep, t->n_int, idx, n, iw) : std::vector<uint32_t>();
     const size_t n_out = b.rhs ? (size_t)n * Hcap : 0;
-    const size_t b_int = (sizeof(uint32_t) * kbits.size() + 15) & ~(size_t)15;
-    const size_t b_rhs = b_int + ((sizeof(uint32_t) * ibits.size() + 15) & ~(size_t)15);
-    const size_t b_vrow = b_rhs + sizeof(double) * n_out;
-    rc = batch_scratch(t, b_vrow + sizeof(int) * n_out);
+    ScratchLayout L;
+    const size_t b_keep = L.take(sizeof(uint32_t) * kbits.size()), b_int = L.take(sizeof(uint32_t) * ibits.size());
+    const size_t b_rhs = L.take(sizeof(double) * n_out), b_vrow = L.take(sizeof(int) * n_out);
+    rc = batch_scratch(t, L.bytes);
     if (rc) return rc;
     char *base = (char *)t->d_scratch;
     cudaStream_t s = t->ctx->stream;
-    CK(cudaMemcpyAsync(base, kbits.data(), sizeof(uint32_t) * kbits.size(), cudaMemcpyHostToDevice, s));
-    nb.keep = (const uint32_t *)base; nb.keep_words = kw;
+    CK(cudaMemcpyAsync(base + b_keep, kbits.data(), sizeof(uint32_t) * kbits.size(), cudaMemcpyHostToDevice, s));
+    nb.keep = (const uint32_t *)(base + b_keep); nb.keep_words = kw;
     if (b.int_keep) {
         CK(cudaMemcpyAsync(base + b_int, ibits.data(), sizeof(uint32_t) * ibits.size(), cudaMemcpyHostToDevice, s));
         nb.int_keep = (const uint32_t *)(base + b_int); nb.int_words = iw;
@@ -172,16 +173,14 @@ static int subset_resident(jslp_tab *t, const SubsetBatch &b, const int *idx, in
     std::vector<int32_t> vrow(n_out);
     rc = batch_launch<NODE_CONFLICT>(t, nb, n, smem, rhs.data(), vrow.data());
     if (rc) return rc;
-    bool need_full = false;
-    for (int k = 0; k < n; k++) need_full |= rb.h_out[k].r.log_n > NODE_LOG_HEAD;
-    rc = batch_fetch_logs(t, n, need_full);
+    // phase 1 keeps its own history (simplex.ts:27): every entry of these logs is a phase-1 entry
+    std::vector<int> hit;
+    rc = batch_screen(t, n, [](int) { return true; }, hit);
     if (rc) return rc;
     for (int k = 0; k < n; k++) {
         const NodeResult &r = rb.h_out[k].r;
         const int i = idx[k];
-        // phase 1 keeps its own history (simplex.ts:27): every entry of this log is a phase-1 entry
-        const int hit_at = first_cycle(batch_log(t, k), std::min(r.log_n, t->node_log_cap));
-        if (hit_at >= 0) { b.set(i, SUBSET_CYCLED, 0, -1, 0.0, hit_at); continue; }
+        if (hit[k] >= 0) { b.set(i, SUBSET_CYCLED, 0, -1, 0.0, hit[k]); continue; }
         if (r.overflow) { redo.push_back(i); continue; }
         const int st = r.status == ST_P1_DONE ? SUBSET_FEASIBLE : SUBSET_INFEASIBLE;
         b.set(i, st, r.is_integral, r.branch_var, r.branch_value, r.p1);
@@ -192,23 +191,15 @@ static int subset_resident(jslp_tab *t, const SubsetBatch &b, const int *idx, in
     return JSLP_OK;
 }
 
-// Every node of b: those whose height fits shared memory on the node kernel, the rest (and the redo) on the single
-// tableau.  The column outputs bound a launch (batch_chunk of the tallest node); without them every resident node runs
-// in one launch.  The snapshot and the caller's scalar state are restored at the end.
+// Every node of b, routed by batch_route on its height.  Only the column outputs bound a launch: without them every
+// resident node runs in one.  The snapshot and the caller's scalar state are restored at the end.
 static int subset_batch(jslp_tab *t, int n_nodes, const SubsetBatch &b) {
     CK(cudaSetDevice(t->ctx->device));
     const CallerState caller(t);
-    std::vector<int> res, redo;
-    int hmax = 1;
-    for (int i = 0; i < n_nodes; i++) {
-        if (batch_resident(t, b.height[i])) { res.push_back(i); hmax = std::max(hmax, b.height[i]); }
-        else redo.push_back(i);
-    }
-    int rc = JSLP_OK;
-    const size_t chunk = b.rhs ? (size_t)batch_chunk(hmax) : std::max<size_t>(1, res.size());
-    for (size_t k0 = 0; k0 < res.size() && rc == JSLP_OK; k0 += chunk)
-        rc = subset_resident(t, b, res.data() + k0, (int)std::min(chunk, res.size() - k0), redo);
-    for (size_t k = 0; k < redo.size() && rc == JSLP_OK; k++) rc = subset_hbm(t, b, redo[k]);
+    int rc = batch_route(
+        t, n_nodes, [&](int i) { return b.height[i]; }, b.rhs != nullptr,
+        [&](const int *idx, int m, std::vector<int> &redo) { return subset_resident(t, b, idx, m, redo); },
+        [&](int i) { return subset_hbm(t, b, i); });
     const int rc2 = jslp_restore(t);  // device-to-device copies, ordered before every later read on the tab's stream
     if (rc == JSLP_OK) rc = rc2;
     caller.restore(t);

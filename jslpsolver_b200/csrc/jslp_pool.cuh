@@ -132,32 +132,30 @@ static int pool_resident(jslp_tab *t, const std::vector<EditDev> &edits, const i
     }
     eoff[n] = f;
     // one device block per chunk: edit offsets, edits, final columns, final labels
-    const size_t b_ed = (sizeof(int) * (size_t)(n + 1) + 15) & ~(size_t)15;
-    const size_t b_rhs = b_ed + ((sizeof(EditDev) * (size_t)tote + 15) & ~(size_t)15);
-    const size_t b_vrow = b_rhs + sizeof(double) * (size_t)n * nb.Hcap;
-    rc = batch_scratch(t, b_vrow + sizeof(int) * (size_t)n * nb.Hcap);
+    const size_t n_out = (size_t)n * nb.Hcap;
+    ScratchLayout L;
+    const size_t b_off = L.take(sizeof(int) * (size_t)(n + 1)), b_ed = L.take(sizeof(EditDev) * (size_t)tote);
+    const size_t b_rhs = L.take(sizeof(double) * n_out), b_vrow = L.take(sizeof(int) * n_out);
+    rc = batch_scratch(t, L.bytes);
     if (rc) return rc;
     char *base = (char *)t->d_scratch;
     cudaStream_t s = t->ctx->stream;
-    CK(cudaMemcpyAsync(base, eoff.data(), sizeof(int) * (size_t)(n + 1), cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(base + b_off, eoff.data(), sizeof(int) * (size_t)(n + 1), cudaMemcpyHostToDevice, s));
     if (tote > 0) CK(cudaMemcpyAsync(base + b_ed, ed.data(), sizeof(EditDev) * (size_t)tote, cudaMemcpyHostToDevice, s));
-    nb.edit_off = (const int *)base;
+    nb.edit_off = (const int *)(base + b_off);
     nb.edits = (const EditDev *)(base + b_ed);
     nb.out_rhs = (double *)(base + b_rhs); nb.out_vrow = (int *)(base + b_vrow);
-    std::vector<double> rhs((size_t)n * nb.Hcap);
-    std::vector<int32_t> vrow((size_t)n * nb.Hcap);
+    std::vector<double> rhs(n_out);
+    std::vector<int32_t> vrow(n_out);
     rc = batch_launch<NODE_POOL>(t, nb, n, smem, rhs.data(), vrow.data());
     if (rc) return rc;
-    bool need_full = false;
-    for (int k = 0; k < n; k++) need_full |= check_cycles && !rb.h_out[k].r.overflow && rb.h_out[k].r.log_n > NODE_LOG_HEAD;
-    rc = batch_fetch_logs(t, n, need_full);
+    std::vector<int> hit;
+    rc = batch_screen(t, n, [&](int k) { return check_cycles && !rb.h_out[k].r.overflow; }, hit);
     if (rc) return rc;
     for (int k = 0; k < n; k++) {
         const NodeResult &r = rb.h_out[k].r;
         const int i = idx[k];
-        const bool again =
-            r.overflow || (check_cycles && first_cycle(batch_log(t, k), std::min(r.log_n, t->node_log_cap)) >= 0);
-        if (again) { redo.push_back(i); continue; }
+        if (r.overflow || hit[k] >= 0) { redo.push_back(i); continue; }
         const int st = r.status == ST_OPTIMAL ? POOL_OPTIMAL : r.status == ST_UNBOUNDED ? POOL_UNBOUNDED : POOL_INFEASIBLE;
         o.set(i, st, r.eval_raw, t->precision, r.is_integral, r.branch_var, r.branch_value, r.p1 + r.p2);
         if (o.is_integral[i]) {
@@ -170,31 +168,21 @@ static int pool_resident(jslp_tab *t, const std::vector<EditDev> &edits, const i
 }
 
 // The node LPs of jslp_pool_batch and jslp_target_batch: node i is the snapshot with edits[edit_off[i] ..
-// edit_off[i+1]) and the cut rows cuts[cut_off[i] .. cut_off[i+1]).  Nodes whose rows fit shared memory run in chunks
-// of k_node_batch<NODE_POOL> launches, the others and the redone ones on the single-tableau path; the tableau ends
-// equal to the snapshot, with the caller's scalar state.
+// edit_off[i+1]) and the cut rows cuts[cut_off[i] .. cut_off[i+1]), routed by batch_route on its height (snapshot rows
+// plus cuts); the tableau ends equal to the snapshot, with the caller's scalar state.
 static int pool_run(jslp_tab *t, const std::vector<EditDev> &edits, const int32_t *edit_off, const jslp_cut *cuts,
                     const int32_t *cut_off, int n_nodes, int check_cycles, PoolOut &o) {
     CK(cudaSetDevice(t->ctx->device));
-    const int H0 = t->saved.H;
     const CallerState caller(t);
-    std::vector<int> res, redo;
-    int maxc = 0;
-    for (int i = 0; i < n_nodes; i++) {
-        const int nc = cut_off[i + 1] - cut_off[i];
-        if (batch_resident(t, H0 + nc)) { res.push_back(i); maxc = std::max(maxc, nc); }
-        else redo.push_back(i);
-    }
-    int rc = JSLP_OK;
-    const int chunk = batch_chunk(H0 + maxc);
-    for (size_t k0 = 0; k0 < res.size() && rc == JSLP_OK; k0 += chunk)
-        rc = pool_resident(t, edits, edit_off, cuts, cut_off, res.data() + k0,
-                           (int)std::min<size_t>(chunk, res.size() - k0), check_cycles, o, redo);
-    for (size_t k = 0; k < redo.size() && rc == JSLP_OK; k++) {
-        const int i = redo[k];
-        rc = pool_hbm(t, edits.data() + edit_off[i], edit_off[i + 1] - edit_off[i], cuts + cut_off[i],
-                      cut_off[i + 1] - cut_off[i], check_cycles, i, o);
-    }
+    int rc = batch_route(
+        t, n_nodes, [&](int i) { return t->saved.H + cut_off[i + 1] - cut_off[i]; }, true,
+        [&](const int *idx, int m, std::vector<int> &redo) {
+            return pool_resident(t, edits, edit_off, cuts, cut_off, idx, m, check_cycles, o, redo);
+        },
+        [&](int i) {
+            return pool_hbm(t, edits.data() + edit_off[i], edit_off[i + 1] - edit_off[i], cuts + cut_off[i],
+                            cut_off[i + 1] - cut_off[i], check_cycles, i, o);
+        });
     const int rc2 = jslp_restore(t);
     if (rc == JSLP_OK) rc = rc2;
     CK(cudaStreamSynchronize(t->ctx->stream));
@@ -212,16 +200,15 @@ static int pool_check(jslp_tab *t, const int32_t *edit_offsets, const jslp_cut *
     if (!t->saved.valid) return fail(JSLP_E_INVALID, what + " needs a snapshot (jslp_save)");
     if (t->nOpt > 0) return fail(JSLP_E_UNSUPPORTED, what + ": optional objectives are not supported");
     if (n_nodes == 0) return JSLP_OK;
-    if (edit_offsets[0] != 0 || cut_offsets[0] != 0) return fail(JSLP_E_INVALID, what + ": offsets[0] must be 0");
-    for (int i = 0; i < n_nodes; i++) {
-        if (edit_offsets[i + 1] < edit_offsets[i] || cut_offsets[i + 1] < cut_offsets[i])
-            return fail(JSLP_E_INVALID, what + ": offsets must not decrease");
+    const int rc = batch_check_offsets({edit_offsets, cut_offsets}, n_nodes, what);
+    if (rc) return rc;
+    for (int i = 0; i < n_nodes; i++)
         if (t->saved.H + cut_offsets[i + 1] - cut_offsets[i] > row_stride)
             return fail(JSLP_E_INVALID, what + ": row_stride is below a " + node + "'s height (rows plus cuts)");
-    }
     return JSLP_OK;
 }
 
+// Every cut row of a batch is a min or max bound on a label of the snapshot.
 static int pool_check_cuts(const jslp_tab *t, const jslp_cut *cuts, int n_cuts, const std::string &what) {
     for (int k = 0; k < n_cuts; k++)
         if ((cuts[k].type != 0 && cuts[k].type != 1) || cuts[k].var_index < 0 || cuts[k].var_index >= t->saved.nVars)

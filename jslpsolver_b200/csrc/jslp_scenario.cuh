@@ -55,10 +55,10 @@ static int scenario_resident(jslp_tab *t, const std::vector<EditDev> &res, const
     if (rc) return rc;
     // one device block per chunk: offsets, edits, final columns, final labels
     const int e0 = offsets[s0], ne = offsets[s0 + n] - e0;
-    const size_t b_off = 0, b_ed = (sizeof(int) * (size_t)(n + 1) + 15) & ~(size_t)15;
-    const size_t b_rhs = b_ed + sizeof(EditDev) * (size_t)ne;
-    const size_t b_vrow = b_rhs + sizeof(double) * (size_t)n * H0;
-    rc = batch_scratch(t, b_vrow + sizeof(int) * (size_t)n * H0);
+    ScratchLayout L;
+    const size_t b_off = L.take(sizeof(int) * (size_t)(n + 1)), b_ed = L.take(sizeof(EditDev) * (size_t)ne);
+    const size_t b_rhs = L.take(sizeof(double) * (size_t)n * H0), b_vrow = L.take(sizeof(int) * (size_t)n * H0);
+    rc = batch_scratch(t, L.bytes);
     if (rc) return rc;
     char *base = (char *)t->d_scratch;
     std::vector<int> off((size_t)n + 1);
@@ -75,15 +75,12 @@ static int scenario_resident(jslp_tab *t, const std::vector<EditDev> &res, const
     }
     rc = batch_launch<NODE_SCENARIO>(t, nb, n, smem, rhs + (size_t)s0 * H0, vrow + (size_t)s0 * H0);
     if (rc) return rc;
-    bool need_full = false;
-    for (int i = 0; i < n; i++) need_full |= check_cycles && !rb.h_out[i].r.overflow && rb.h_out[i].r.log_n > NODE_LOG_HEAD;
-    rc = batch_fetch_logs(t, n, need_full);
+    std::vector<int> hit;
+    rc = batch_screen(t, n, [&](int i) { return check_cycles && !rb.h_out[i].r.overflow; }, hit);
     if (rc) return rc;
     for (int i = 0; i < n; i++) {
         const NodeResult &r = rb.h_out[i].r;
-        const bool again =
-            r.overflow || (check_cycles && first_cycle(batch_log(t, i), std::min(r.log_n, t->node_log_cap)) >= 0);
-        if (again) { redo.push_back(s0 + i); continue; }
+        if (r.overflow || hit[i] >= 0) { redo.push_back(s0 + i); continue; }
         status[s0 + i] = r.status == ST_OPTIMAL ? SCEN_OPTIMAL : r.status == ST_UNBOUNDED ? SCEN_UNBOUNDED : SCEN_INFEASIBLE;
         eval_raw[s0 + i] = r.eval_raw;
         p1[s0 + i] = r.p1;
@@ -100,16 +97,15 @@ extern "C" int jslp_scenario_batch(jslp_tab *t, const jslp_scenario_edit *edits,
         return fail(JSLP_E_INVALID, "scenario_batch: bad offsets / output arguments");
     if (t->nOpt > 0) return fail(JSLP_E_UNSUPPORTED, "scenario_batch: optional objectives are not supported");
     if (n_scenarios == 0) return JSLP_OK;
-    if (offsets[0] != 0) return fail(JSLP_E_INVALID, "scenario_batch: offsets[0] must be 0");
-    for (int i = 0; i < n_scenarios; i++)
-        if (offsets[i + 1] < offsets[i]) return fail(JSLP_E_INVALID, "scenario_batch: offsets must not decrease");
+    int rc = batch_check_offsets({offsets}, n_scenarios, "scenario_batch");
+    if (rc) return rc;
     const int n_edits = offsets[n_scenarios];
     if (n_edits > 0 && !edits) return fail(JSLP_E_INVALID, "scenario_batch: edits is NULL");
     CK(cudaSetDevice(t->ctx->device));
     // updateRightHandSide / updateCost resolved once against the labels: no edit pivots, so the positions are the
     // same for every scenario and every edit of it
     HostMaps m;
-    int rc = load_maps(t, m);
+    rc = load_maps(t, m);
     if (rc) return rc;
     std::vector<EditDev> res((size_t)n_edits);
     for (int i = 0; i < n_scenarios; i++)
@@ -125,21 +121,18 @@ extern "C" int jslp_scenario_batch(jslp_tab *t, const jslp_scenario_edit *edits,
     if (rc) return rc;
     rc = snapshot_copy(t, 2, true);
     if (rc) return rc;
-    std::vector<int> redo;
-    if (batch_resident(t, t->H)) {
-        const int chunk = batch_chunk(t->H);
-        for (int s0 = 0; s0 < n_scenarios && rc == JSLP_OK; s0 += chunk)
-            rc = scenario_resident(t, res, offsets, s0, std::min(chunk, n_scenarios - s0), check_cycles, status, eval_raw,
-                                   p1, p2, rhs, vrow, redo);
-    } else {
-        for (int i = 0; i < n_scenarios; i++) redo.push_back(i);
-    }
+    // every scenario has the tab's height, so either all of them are resident or none, and a launch's are consecutive
     const int H = t->H;
-    for (size_t k = 0; k < redo.size() && rc == JSLP_OK; k++) {
-        const int i = redo[k];
-        rc = scenario_sequential(t, edits + offsets[i], offsets[i + 1] - offsets[i], check_cycles, status + i,
-                                 eval_raw + i, p1 + i, p2 + i, rhs + (size_t)i * H, vrow + (size_t)i * H);
-    }
+    rc = batch_route(
+        t, n_scenarios, [&](int) { return H; }, true,
+        [&](const int *idx, int m, std::vector<int> &redo) {
+            return scenario_resident(t, res, offsets, idx[0], m, check_cycles, status, eval_raw, p1, p2, rhs, vrow,
+                                     redo);
+        },
+        [&](int i) {
+            return scenario_sequential(t, edits + offsets[i], offsets[i + 1] - offsets[i], check_cycles, status + i,
+                                       eval_raw + i, p1 + i, p2 + i, rhs + (size_t)i * H, vrow + (size_t)i * H);
+        });
     // the caller's tableau, labels, staged pivot and record exactly as they were
     const int rc2 = snapshot_copy(t, 2, false);
     if (rc == JSLP_OK) rc = rc2;
