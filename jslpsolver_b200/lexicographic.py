@@ -21,24 +21,32 @@ from .variability import _gap, _point
 WHAT = "Lexicographic()"
 
 
-def _objectives(model: dict):
+def _objectives(model: dict, what: str = WHAT):
     opt = model.get("optimize")
     keys = object_keys(opt) if isinstance(opt, dict) else []
     if len(keys) < 2:
-        raise ValueError(f"{WHAT} needs `optimize` with at least two objectives in priority order, e.g. "
+        raise ValueError(f"{what} needs `optimize` with at least two objectives in priority order, e.g. "
                          "{\"a\": \"max\", \"b\": \"min\"}")
     return keys, {k: "max" if opt[k] == "max" else "min" for k in keys}
 
 
-def _gaps(name: str, x, keys) -> list:
+def _gaps(name: str, x, keys, what: str = WHAT) -> list:
     """gap= / absolute_gap= as one float per level: a number applies to every level, a dict {objective: number} to
     the objectives it names (0 for the others)."""
     if isinstance(x, dict):
         for k in x:
             if k not in keys:
-                raise ValueError(f"{WHAT}: {name}= names {k!r}, which is not an objective of `optimize`")
-        return [_gap(name, x[k], WHAT) if k in x else 0.0 for k in keys]
-    return [_gap(name, x, WHAT)] * len(keys)
+                raise ValueError(f"{what}: {name}= names {k!r}, which is not an objective of `optimize`")
+        return [_gap(name, x[k], what) if k in x else 0.0 for k in keys]
+    return [_gap(name, x, what)] * len(keys)
+
+
+def allowance(key: str, gap: float, absolute_gap: float, z: float, what: str = WHAT) -> float:
+    """t_k = max(absolute_gap_k, gap_k * |z_k|), refused when it overflows to infinity."""
+    t = max(absolute_gap, gap * abs(z))
+    if math.isinf(t):
+        raise ValueError(f"{what}: the allowance of {key!r} overflows (gap={gap!r}, optimum={z!r})")
+    return t
 
 
 def Lexicographic(solver, model: Any, gap=0.0, absolute_gap=0.0, precision: Optional[float] = None,
@@ -111,10 +119,7 @@ def Lexicographic(solver, model: Any, gap=0.0, absolute_gap=0.0, precision: Opti
                 plan = tuple(point[v.id] for v in instance.variables)
             levels[k]["optimum"] = z
             if k + 1 < len(keys):
-                t = max(absolute[k], gaps[k] * abs(z))
-                if math.isinf(t):
-                    raise ValueError(f"{WHAT}: the allowance of {key!r} overflows (gap={gaps[k]!r}, optimum={z!r})")
-                levels[k]["allowance"] = t
+                levels[k]["allowance"] = allowance(key, gaps[k], absolute[k], z)
     finally:
         if cur is not None and cur is not instance.tableau:
             cur.close()

@@ -31,19 +31,28 @@ def _refuse(model: dict) -> None:
         raise ValueError(f"{WHAT} takes a JSON model")
     if model.get("external"):
         raise ValueError(f"{WHAT} does not support external solvers: solve the model with its own solver")
-    if not (any(_truthy(v) for v in (model.get("ints") or {}).values()) or
-            any(_truthy(v) for v in (model.get("binaries") or {}).values())):
-        raise ValueError(f"{WHAT} needs integer or binary variables: for a continuous LP use "
-                         "Solve(model, full=True).variability()")
-    for spec in (model.get("constraints") or {}).values():
-        if isinstance(spec, dict) and (spec.get("weight") is not None or spec.get("priority") is not None):
-            raise ValueError(f"{WHAT} does not support soft constraints (weight / priority): make them hard rows")
+    refuse_non_mip(model, WHAT, "Solve(model, full=True).variability()")
     opt = model.get("optimize")
     if isinstance(opt, dict) and len(object_keys(opt)) > 1:
         raise ValueError(f"{WHAT} takes one objective: `optimize` has {len(object_keys(opt))}; use Lexicographic() "
                          "or Solve() for several")
+    refuse_unrestricted(model, WHAT)
+
+
+def refuse_non_mip(model: dict, what: str, continuous: str) -> None:
+    """The refusals of the MIP analyses that search on a bound tableau: a model without integer or binary variables
+    (`continuous` names what answers it for a continuous LP) and soft constraints."""
+    if not (any(_truthy(v) for v in (model.get("ints") or {}).values()) or
+            any(_truthy(v) for v in (model.get("binaries") or {}).values())):
+        raise ValueError(f"{what} needs integer or binary variables: for a continuous LP use {continuous}")
+    for spec in (model.get("constraints") or {}).values():
+        if isinstance(spec, dict) and (spec.get("weight") is not None or spec.get("priority") is not None):
+            raise ValueError(f"{what} does not support soft constraints (weight / priority): make them hard rows")
+
+
+def refuse_unrestricted(model: dict, what: str) -> None:
     if any(_truthy(v) for v in (model.get("unrestricted") or {}).values()):
-        raise ValueError(f"{WHAT} does not support unrestricted variables: re-solving from an optimum where one is "
+        raise ValueError(f"{what} does not support unrestricted variables: re-solving from an optimum where one is "
                          "basic and negative starts with phase-1 pivots; split each into two restricted variables")
 
 
@@ -88,10 +97,13 @@ class _Search:
 
 def run(evaluate, targets, start: list, P: float, max_nodes: int, width: Optional[int], wave: int = 1) -> dict:
     """The concurrent target searches of DESIGN.md section 2o (rules 4 to 8).  targets = [(label, sense, integer)];
-    start[k] = target k's incumbent value at x*.  evaluate([(k, cuts), ...]) -> [Node, ...], the nodes' LPs on the
-    bound tableau with row 0 set to -s_k on label_k.  Each round evaluates the children of the first `width` open nodes
-    (None: wave // live searches, at least 1) of every live search in one call, then commits the searches in target
-    order.  Returns {"best", "witness" (Node or None: x*), "state", "bound", "nodes", "lps", "rounds"}."""
+    a label of None stands for the node LP's own objective, so its value at an integral node is the node's evaluation
+    and its sense is -1 (the lexicographic levels of section 2q).  start[k] = target k's incumbent value at x*; a
+    target without one starts at -s * math.inf (math.inf for a min target, such as the label-None target).
+    evaluate([(k, cuts), ...]) -> [Node, ...], the nodes' LPs on the bound tableau with row 0 set to -s_k on label_k.
+    Each round evaluates the children of the first `width` open nodes (None: wave // live searches, at least 1) of
+    every live search in one call, then commits the searches in target order.  Returns {"best", "witness" (Node or
+    None: x*), "state", "bound", "nodes", "lps", "rounds"}."""
     n = len(targets)
     searches = [_Search(k, lab, s, integer) for k, (lab, s, integer) in enumerate(targets)]
     best, witness = list(start), [None] * n
@@ -102,7 +114,7 @@ def run(evaluate, targets, start: list, P: float, max_nodes: int, width: Optiona
     def share(node: Node) -> None:
         at = plan_values(node.rhs, node.vrow)
         for sr in searches:
-            v = at.get(sr.label, 0.0)
+            v = node.evaluation if sr.label is None else at.get(sr.label, 0.0)
             if beats(sr, v):
                 best[sr.k], witness[sr.k] = v, node
 

@@ -8,6 +8,7 @@ from . import validation
 from .conflict import Conflict as _conflict
 from .frontier import Frontier as _frontier
 from .lexicographic import Lexicographic as _lexicographic
+from .lexicographic_mip import LexicographicMIP as _lexicographic_mip
 from .mip_scenarios import Scenarios as _scenarios
 from .mip_variability import Variability as _variability
 from .model import Model, object_keys
@@ -74,6 +75,13 @@ class Solver:
         """Hierarchical objectives of a continuous LP: the objectives of `optimize` in order, each optimised over the
         plans within an allowance of every earlier optimum (lexicographic.py, DESIGN.md section 2j)."""
         return _lexicographic(self, model, gap, absolute_gap, precision, validate)
+
+    def LexicographicMIP(self, model: dict, gap=0.0, absolute_gap=0.0, max_nodes=10000, width=None,
+                         precision: Optional[float] = None, validate: bool = False) -> dict:
+        """Hierarchical objectives of a MIP: the objectives of `optimize` in order, each optimised exactly over the
+        integer plans within an allowance of every earlier optimum, one branch and bound per level
+        (lexicographic_mip.py, DESIGN.md section 2q).  `width` tunes the batching only."""
+        return _lexicographic_mip(self, model, gap, absolute_gap, max_nodes, width, precision, validate)
 
     def Repair(self, model: dict, weights=None, *, objective: bool = True, gap=0.0, absolute_gap=0.0,
                precision: Optional[float] = None, validate: bool = False) -> dict:
@@ -166,6 +174,11 @@ def Frontier(model: dict, precision: Optional[float] = None, validate: bool = Fa
 def Lexicographic(model: dict, gap=0.0, absolute_gap=0.0, precision: Optional[float] = None,
                   validate: bool = False) -> dict:
     return solver.Lexicographic(model, gap, absolute_gap, precision, validate)
+
+
+def LexicographicMIP(model: dict, gap=0.0, absolute_gap=0.0, max_nodes=10000, width=None,
+                     precision: Optional[float] = None, validate: bool = False) -> dict:
+    return solver.LexicographicMIP(model, gap, absolute_gap, max_nodes, width, precision, validate)
 
 
 def Repair(model: dict, weights=None, *, objective: bool = True, gap=0.0, absolute_gap=0.0,
