@@ -48,6 +48,36 @@ def search(evaluate, P: float, max_nodes: int, width: Optional[int], wave: int) 
             "rounds": out["rounds"]}
 
 
+def run_stage(cur, entry: dict, P: float, max_nodes: int, width: Optional[int], n_ints: int) -> dict:
+    """Rule 2 on the tableau cur: its snapshot saved, then search() with every node LP one jslp_pool_batch region (no
+    fixings, the node's cut rows, cycle check on) and the default width one wave of cur plus an 8-level dive.  The
+    node LPs' pivots and the search's nodes, LPs and rounds go into entry."""
+    def evaluate(specs):
+        res = cur.pool_batch([([], cuts) for _, cuts in specs], check_cycles=True)
+        entry["pivots"] += int(res["pivots"].sum())
+        return [node_of(res, i, cur.height, cuts) for i, (_, cuts) in enumerate(specs)]
+
+    cur.save()
+    found = search(evaluate, P, max_nodes, width, iis.wave_width(cur.context, cur.height + min(n_ints, 8), cur.width))
+    entry.update(nodes=found["nodes"], lps=found["lps"], rounds=found["rounds"])
+    return found
+
+
+def delta(cur, entry: dict, best, what: str) -> Optional[float]:
+    """Rule 1's R_k and Delta_k: cur restored and its root LP solved (cycle check on), its pivots added to entry;
+    Delta_k = max(0, raw M[0,0] of the optimal node best - raw M[0,0] of R_k), or None when the root LP cycled.
+    `what` names the root LP in the RuntimeError raised when it has no optimum."""
+    cur.restore()
+    cur.simplex(check_cycles=True)
+    st = cur.lastStatus
+    entry["pivots"] += int(st.phase1_pivots) + int(st.phase2_pivots)
+    if st.cycled:
+        return None
+    if not (cur.feasible and cur.bounded):
+        raise RuntimeError(f"{what} has no optimum, but its search found one")
+    return max(0.0, float(best.rhs[0]) - float(cur.final_state()[1][0]))
+
+
 def signed(sense: str, raw: float) -> float:
     """The objective value of a raw M[0,0] (the tableau minimises, so a max objective's row holds -value)."""
     return (-raw if sense == "max" else raw) + 0.0
@@ -85,12 +115,6 @@ def LexicographicMIP(solver, model: Any, gap=0.0, absolute_gap=0.0, max_nodes=10
     out = {"feasible": True, "bounded": True, "stop": "reached", "objectives": None, "values": None,
            "levels": levels}
     plan, cur, arg = None, None, 0.0
-
-    def evaluate(specs):
-        res = cur.pool_batch([([], cuts) for _, cuts in specs], check_cycles=True)
-        lv["pivots"] += int(res["pivots"].sum())
-        return [node_of(res, i, cur.height, cuts) for i, (_, cuts) in enumerate(specs)]
-
     try:
         tab.setModel(instance)
         launches0 = tab.context.launches
@@ -108,10 +132,7 @@ def LexicographicMIP(solver, model: Any, gap=0.0, absolute_gap=0.0, max_nodes=10
             else:
                 lv.update(kind="initial" if k == 0 else "face" if arg == 0.0 else "bound", width=cur.width,
                           height=cur.height)
-                cur.save()
-                found = search(evaluate, P, max_nodes, width,
-                               iis.wave_width(cur.context, cur.height + min(n_ints, 8), cur.width))
-                lv.update(nodes=found["nodes"], lps=found["lps"], rounds=found["rounds"])
+                found = run_stage(cur, lv, P, max_nodes, width, n_ints)
                 state, best = found["state"], found["witness"]
                 if state in ("unbounded", "cycled"):
                     out["stop"] = state
@@ -139,17 +160,11 @@ def LexicographicMIP(solver, model: Any, gap=0.0, absolute_gap=0.0, max_nodes=10
             if k + 1 < len(keys):
                 lv["allowance"] = t = allowance(key, gaps[k], absolute[k], lv["optimum"], WHAT)
                 if cur is not None:  # R_k and Delta_k
-                    cur.restore()
-                    cur.simplex(check_cycles=True)
-                    st = cur.lastStatus
-                    lv["pivots"] += int(st.phase1_pivots) + int(st.phase2_pivots)
-                    if st.cycled:
+                    d = delta(cur, lv, best, f"{WHAT}: the root LP of level {k + 1} ({key!r})")
+                    if d is None:
                         out["stop"] = "cycled"
                         break
-                    if not (cur.feasible and cur.bounded):
-                        raise RuntimeError(f"{WHAT}: the root LP of level {k + 1} ({key!r}) has no optimum, but its "
-                                           "search found one")
-                    arg = t + max(0.0, float(best.rhs[0]) - float(cur.final_state()[1][0]))
+                    arg = t + d
         out["launches"] = tab.context.launches - launches0
     finally:
         if cur is not None and cur is not tab:

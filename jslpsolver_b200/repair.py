@@ -28,16 +28,16 @@ PICK = "give {'min': ..., 'max': ...}"
 MAX_WIDTH = 25600  # the pivot step stages a whole row in shared memory (jslp_tab_create refuses wider tableaux)
 
 
-def _weight(x, what: str) -> float:
+def _weight(x, what: str, caller: str = WHAT) -> float:
     if isinstance(x, bool) or not isinstance(x, numbers.Real):
-        raise ValueError(f"{WHAT}: {what} must be a number, not {type(x).__name__}")
+        raise ValueError(f"{caller}: {what} must be a number, not {type(x).__name__}")
     x = float(x)
     if not (math.isfinite(x) and x > 0.0):
-        raise ValueError(f"{WHAT}: {what} must be finite and > 0, not {x!r}")
+        raise ValueError(f"{caller}: {what} must be finite and > 0, not {x!r}")
     return x
 
 
-def relaxable_rows(m, weights) -> tuple:
+def relaxable_rows(m, weights, what: str = WHAT) -> tuple:
     """(rows, weights): the tableau rows (1-based, increasing) that may be relaxed and their weights.  weights=None
     relaxes every row with weight 1; a dict {name: w} relaxes the rows of the constraints it names, `w` a number for
     every row of that constraint or {"min": a, "max": b} per side, as scenarios() reads a right-hand side."""
@@ -45,23 +45,23 @@ def relaxable_rows(m, weights) -> tuple:
     if weights is None:
         return list(range(1, len(m.constraints) + 1)), [1.0] * len(m.constraints)
     if not isinstance(weights, dict):
-        raise ValueError(f"{WHAT}: weights= takes a dict of constraint name -> weight, not {type(weights).__name__}")
+        raise ValueError(f"{what}: weights= takes a dict of constraint name -> weight, not {type(weights).__name__}")
     chosen = {}
     for name, value in weights.items():
         if isinstance(value, dict):
             if not value:
-                raise ValueError(f"{WHAT}: constraint {name!r}: the dict needs a 'min' and / or a 'max' key")
+                raise ValueError(f"{what}: constraint {name!r}: the dict needs a 'min' and / or a 'max' key")
             for side, v in value.items():
                 if side not in ("min", "max"):
-                    raise ValueError(f"{WHAT}: constraint {name!r}: side must be 'min' or 'max', not {side!r}")
-                w = _weight(v, f"the {side} weight of {name!r}")
-                for label in _constraint_rows(m, name, side, WHAT, PICK)[0]:
+                    raise ValueError(f"{what}: constraint {name!r}: side must be 'min' or 'max', not {side!r}")
+                w = _weight(v, f"the {side} weight of {name!r}", what)
+                for label in _constraint_rows(m, name, side, what, PICK)[0]:
                     chosen[row_of[label]] = w
         else:
             labels = [c.index for c in m.constraints if (c.name if c.name is not None else c.index) == name]
             if not labels:
-                raise ValueError(f"{WHAT}: no constraint named {name!r}")
-            w = _weight(value, f"the weight of {name!r}")
+                raise ValueError(f"{what}: no constraint named {name!r}")
+            w = _weight(value, f"the weight of {name!r}", what)
             for label in labels:
                 chosen[row_of[label]] = w
     rows = sorted(chosen)
@@ -81,6 +81,51 @@ def _vertex(rhs, vrow) -> dict:
     return {int(vrow[r]): float(rhs[r]) for r in range(1, len(vrow))}
 
 
+def one_objective(model: dict, what: str = WHAT) -> dict:
+    """The model with a one-key `optimize` dict written as `optimize` / `opType`; several keys are refused."""
+    opt = model.get("optimize")
+    if isinstance(opt, dict):
+        keys = object_keys(opt)
+        if len(keys) > 1:
+            raise ValueError(f"{what} takes one objective: `optimize` has {len(keys)}")
+        if keys:
+            model = dict(model, optimize=keys[0], opType="max" if opt[keys[0]] == "max" else "min")
+    return model
+
+
+def check_width(W: int, k: int, what: str = WHAT) -> None:
+    """Refuses an elastic tableau of W + k columns beyond the pivot step's cap."""
+    if W + k > MAX_WIDTH:
+        raise ValueError(f"{what}: the elastic tableau needs {W + k} columns ({W} of the model and "
+                         f"{k} violations), beyond the pivot step's cap of {MAX_WIDTH} columns")
+
+
+def allowance(gap: float, absolute_gap: float, vstar: float, what: str = WHAT) -> float:
+    """Stage 2's t = max(absolute_gap, gap * V*), refused when it overflows to infinity."""
+    t = max(absolute_gap, gap * abs(vstar))
+    if math.isinf(t):
+        raise ValueError(f"{what}: the allowance gap * V* overflows (gap={gap!r}, V*={vstar!r})")
+    return t
+
+
+def report(out: dict, instance, model: dict, key, rows, w, plan, e) -> None:
+    """Fills out's "violation" (sum w_j e_j in row order), "constraints" (the rows with e_j > P, their repaired
+    right-hand sides), "values" and "result" from a plan and the violations e_j of the relaxable rows."""
+    violation = 0.0
+    for wj, ej in zip(w, e):
+        violation += wj * ej
+    out["violation"] = violation
+    for r, wj, ej in zip(rows, w, e):
+        if ej > instance.precision:
+            con = instance.constraints[r - 1]
+            upper = con.isUpperBound
+            out["constraints"].append({"name": con.name if con.name is not None else con.index,
+                                       "type": "max" if upper else "min", "rhs": con.rhs, "weight": wj,
+                                       "violation": ej, "repairedRhs": con.rhs + ej if upper else con.rhs - ej})
+    out["values"] = {v.id: x for v, x in zip(instance.variables, plan)}
+    out["result"] = objective_sums(instance, model, [key], plan)[key]
+
+
 def Repair(solver, model: Any, weights=None, *, objective: bool = True, gap=0.0, absolute_gap=0.0,
            precision: Optional[float] = None, validate: bool = False) -> dict:
     """See the module docstring.  `solver` supplies the engine settings of the tableau (Solver._instance)."""
@@ -92,13 +137,7 @@ def Repair(solver, model: Any, weights=None, *, objective: bool = True, gap=0.0,
         raise ValueError(f"{WHAT} takes a JSON model")
     if model.get("external"):
         raise ValueError(f"{WHAT} does not support external solvers")
-    opt = model.get("optimize")
-    if isinstance(opt, dict):
-        keys = object_keys(opt)
-        if len(keys) > 1:
-            raise ValueError(f"{WHAT} takes one objective: `optimize` has {len(keys)}")
-        if keys:
-            model = dict(model, optimize=keys[0], opType="max" if opt[keys[0]] == "max" else "min")
+    model = one_objective(model)
     _refuse(model, WHAT)
     if any(_truthy(v) for v in (model.get("unrestricted") or {}).values()):
         raise ValueError(f"{WHAT} does not support unrestricted variables: re-solving from an optimum where one is "
@@ -109,9 +148,7 @@ def Repair(solver, model: Any, weights=None, *, objective: bool = True, gap=0.0,
     rows, w = relaxable_rows(instance, weights)
     it = instance.initial_tableau()
     H, W = it.matrix.shape
-    if W + len(rows) > MAX_WIDTH:
-        raise ValueError(f"{WHAT}: the elastic tableau needs {W + len(rows)} columns ({W} of the model and "
-                         f"{len(rows)} violations), beyond the pivot step's cap of {MAX_WIDTH} columns")
+    check_width(W, len(rows))
     sigma = -1.0 if instance.isMinimization else 1.0
     key = model.get("optimize") if isinstance(model.get("optimize"), str) else None
     first = H + W - 2  # l*: the first violation label of a freshly uploaded tableau
@@ -147,9 +184,7 @@ def Repair(solver, model: Any, weights=None, *, objective: bool = True, gap=0.0,
         s1["optimum"] = vstar
         plan, e = plan_of(_vertex(rhs, vrow))
         if objective:
-            t = max(absolute_gap, gap * abs(vstar))
-            if math.isinf(t):
-                raise ValueError(f"{WHAT}: the allowance gap * V* overflows (gap={gap!r}, V*={vstar!r})")
+            t = allowance(gap, absolute_gap, vstar)
             s2 = {"kind": "face" if t == 0.0 else "bound", "allowance": t, "optimum": None, "pivots": 0,
                   "width": None, "height": None}
             out["stages"].append(s2)
@@ -176,17 +211,5 @@ def Repair(solver, model: Any, weights=None, *, objective: bool = True, gap=0.0,
         for tab in (nxt, E, parent):
             if tab is not None:
                 tab.close()
-    violation = 0.0
-    for wj, ej in zip(w, e):
-        violation += wj * ej
-    out["violation"] = violation
-    for r, wj, ej in zip(rows, w, e):
-        if ej > instance.precision:
-            con = instance.constraints[r - 1]
-            upper = con.isUpperBound
-            out["constraints"].append({"name": con.name if con.name is not None else con.index,
-                                       "type": "max" if upper else "min", "rhs": con.rhs, "weight": wj,
-                                       "violation": ej, "repairedRhs": con.rhs + ej if upper else con.rhs - ej})
-    out["values"] = {v.id: x for v, x in zip(instance.variables, plan)}
-    out["result"] = objective_sums(instance, model, [key], plan)[key]
+    report(out, instance, model, key, rows, w, plan, e)
     return out

@@ -15,6 +15,7 @@ from .model import Model, object_keys
 from .polyopt import Polyopt
 from .pool import Pool as _pool
 from .repair import Repair as _repair
+from .repair_mip import RepairMIP as _repair_mip
 
 
 class Solver:
@@ -89,6 +90,14 @@ class Solver:
         optimised over the plans that reach it (repair.py, DESIGN.md section 2k)."""
         return _repair(self, model, weights, objective=objective, gap=gap, absolute_gap=absolute_gap,
                        precision=precision, validate=validate)
+
+    def RepairMIP(self, model: dict, weights=None, *, objective: bool = True, gap=0.0, absolute_gap=0.0,
+                  max_nodes=10000, width=None, precision: Optional[float] = None, validate: bool = False) -> dict:
+        """The least weighted relaxation of the rows of a (possibly infeasible) MIP over integer plans, then its
+        objective optimised over the integer plans that reach it, each stage an exact branch and bound
+        (repair_mip.py, DESIGN.md section 2r).  `width` tunes the batching only."""
+        return _repair_mip(self, model, weights, objective=objective, gap=gap, absolute_gap=absolute_gap,
+                           max_nodes=max_nodes, width=width, precision=precision, validate=validate)
 
     def Pool(self, model: dict, k=10, gap=0.0, absolute_gap=0.0, precision: Optional[float] = None,
              validate: bool = False, max_nodes=100000, width=None) -> dict:
@@ -185,6 +194,12 @@ def Repair(model: dict, weights=None, *, objective: bool = True, gap=0.0, absolu
            precision: Optional[float] = None, validate: bool = False) -> dict:
     return solver.Repair(model, weights, objective=objective, gap=gap, absolute_gap=absolute_gap,
                          precision=precision, validate=validate)
+
+
+def RepairMIP(model: dict, weights=None, *, objective: bool = True, gap=0.0, absolute_gap=0.0, max_nodes=10000,
+              width=None, precision: Optional[float] = None, validate: bool = False) -> dict:
+    return solver.RepairMIP(model, weights, objective=objective, gap=gap, absolute_gap=absolute_gap,
+                            max_nodes=max_nodes, width=width, precision=precision, validate=validate)
 
 
 def Pool(model: dict, k=10, gap=0.0, absolute_gap=0.0, precision: Optional[float] = None, validate: bool = False,
