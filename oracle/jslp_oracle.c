@@ -840,6 +840,9 @@ void orc_dm_add_constraint(orc_tab *t, int isUpperBound, double rhs, int slackIn
         }
     }
     ensure_maps(t, slackIndex + 1);
+    /* the caller's index came from Tableau.getNewElementIndex (model.ts:103-124), which advanced lastElementIndex:
+       branching cuts added later must not reuse it */
+    if (slackIndex + 1 > t->lastElementIndex) t->lastElementIndex = slackIndex + 1;
     t->vrow[lastRow] = slackIndex;
     t->rowOf[slackIndex] = lastRow;
     t->colOf[slackIndex] = -1;
@@ -863,7 +866,7 @@ int orc_dm_remove_constraint(orc_tab *t, int slackIndex) {
 }
 
 /* :253-302; costEntry = (isMinimization ? -cost : cost); optSlot = -1 for priority 0 */
-void orc_dm_add_variable(orc_tab *t, int varIndex, double costEntry, int optSlot) {
+void orc_dm_add_variable(orc_tab *t, int varIndex, double costEntry, int optSlot, int isInteger, int isUnrestricted) {
     const int oldW = t->W, newW = oldW + 1, H = t->H;
     double *nm = (double *)calloc((size_t)(t->capRows > H ? t->capRows : H) * newW, sizeof(double));
     for (int r = 0; r < H; r++) memcpy(nm + (size_t)r * newW, t->M + (size_t)r * oldW, sizeof(double) * oldW);
@@ -882,13 +885,30 @@ void orc_dm_add_variable(orc_tab *t, int varIndex, double costEntry, int optSlot
     if (optSlot < 0) t->M[lastColumn] = costEntry;
     else { t->optRC[(size_t)optSlot * newW + lastColumn] = costEntry; t->M[lastColumn] = 0; }
     ensure_maps(t, varIndex + 1);
+    if (varIndex + 1 > t->lastElementIndex) t->lastElementIndex = varIndex + 1;  /* getNewElementIndex (model.ts:163) */
     t->colOf[varIndex] = lastColumn;
     t->vcol[lastColumn] = varIndex;
+    /* Model.addVariable (model.ts:169-187): integerVariables.push, unrestrictedVariables[varIndex] = true */
+    if (isInteger) {
+        t->intVars = (int *)realloc(t->intVars, sizeof(int) * (size_t)(t->nInt + 1));
+        t->intVars[t->nInt++] = varIndex;
+    }
+    if (isUnrestricted) {
+        if (varIndex >= t->unresN) {
+            t->unres = (unsigned char *)realloc(t->unres, (size_t)varIndex + 1);
+            memset(t->unres + t->unresN, 0, (size_t)(varIndex + 1 - t->unresN));
+            t->unresN = varIndex + 1;
+        }
+        t->unres[varIndex] = 1;
+    }
 }
 
 /* :304-316 (the stride stays width: the reference only decrements `width`, leaving the matrix layout at the old
    width -- every later access uses the NEW width as stride, i.e. the reference's tableau is scrambled after this
-   call unless the removed column was the last one; restated literally) */
+   call unless the removed column was the last one; restated literally).  The optional objectives are another
+   matter: the reference keeps one reducedCosts array per objective, indexed by column alone, so a narrower width
+   moves none of them.  Here they share one nOpt x W block, so each row is compacted to the new width to keep
+   objective o at o * (W - 1), where separate arrays would leave its entries. */
 int orc_dm_remove_variable(orc_tab *t, int varIndex) {
     const int W = t->W, lastColumn = W - 1;
     const int c = orc_dm_take_out_of_base(t, varIndex);
@@ -897,6 +917,8 @@ int orc_dm_remove_variable(orc_tab *t, int varIndex) {
     t->vcol[c] = t->vcol[lastColumn];
     t->rowOf[varIndex] = -1;
     t->colOf[varIndex] = -1;
+    for (int o = 1; o < t->nOpt; o++)
+        memmove(t->optRC + (size_t)o * (W - 1), t->optRC + (size_t)o * W, sizeof(double) * (size_t)(W - 1));
     t->W -= 1;
     return 0;
 }

@@ -107,7 +107,7 @@ def lib():
         L.orc_dm_update_cost.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_double]
         L.orc_dm_add_constraint.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_double, ctypes.c_int, ctypes.c_void_p,
                                             ctypes.c_void_p, ctypes.c_int]
-        L.orc_dm_add_variable.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_double, ctypes.c_int]
+        L.orc_dm_add_variable.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_double, ctypes.c_int, ctypes.c_int, ctypes.c_int]
         L.orc_add_mir_cut.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int]
         L.orc_add_mir_cut.restype = ctypes.c_int
         L.orc_apply_mir_cuts.argtypes = [ctypes.c_void_p]
@@ -680,8 +680,9 @@ class OracleTableau:
     def remove_constraint(self, slack_index):
         return lib().orc_dm_remove_constraint(self.h, int(slack_index))
 
-    def add_variable(self, var_index, cost_entry, opt_slot=-1):
-        lib().orc_dm_add_variable(self.h, int(var_index), float(cost_entry), int(opt_slot))
+    def add_variable(self, var_index, cost_entry, opt_slot=-1, is_integer=False, is_unrestricted=False):
+        lib().orc_dm_add_variable(self.h, int(var_index), float(cost_entry), int(opt_slot), int(bool(is_integer)),
+                                  int(bool(is_unrestricted)))
         self.W += 1
 
     def remove_variable(self, var_index):
