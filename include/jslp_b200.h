@@ -406,6 +406,19 @@ int jslp_target_batch(jslp_tab *tab, const jslp_scenario_edit *edits, const int3
                       double *evaluation, int32_t *is_integral, int32_t *branch_var, double *branch_value,
                       int32_t *pivots, double *rhs, int32_t *vrow);
 
+/* The node LPs of the box searches behind the Pareto frontier of a two-objective MIP, DESIGN.md section 2s.  Node i is
+ * the saved snapshot (the model's initial tableau with one bound row per objective) with the edits
+ * edits[edit_offsets[i] .. edit_offsets[i+1]) applied in order as jslp_scenario_batch applies them (kind 0 =
+ * updateRightHandSide of the slack label `index`, kind 1 = updateCost of the label `index`, both resolved against the
+ * snapshot's labels; a node's kind-0 edits come before its kind-1 edits; any other kind is JSLP_E_INVALID), then the
+ * cut rows cuts[cut_offsets[i] .. cut_offsets[i+1]) appended as jslp_add_cuts appends them (labels from the snapshot's
+ * lastElementIndex), then simplex() with check_cycles and the isIntegral / getMostFractionalVar scan.  Routing, outputs,
+ * row_stride and the state on return are jslp_target_batch's.  No optional objectives (JSLP_E_UNSUPPORTED). */
+int jslp_box_batch(jslp_tab *tab, const jslp_scenario_edit *edits, const int32_t *edit_offsets, const jslp_cut *cuts,
+                   const int32_t *cut_offsets, int n_nodes, int check_cycles, int row_stride, int32_t *status,
+                   double *evaluation, int32_t *is_integral, int32_t *branch_var, double *branch_value,
+                   int32_t *pivots, double *rhs, int32_t *vrow);
+
 /* The node LPs of the feasibility searches behind a MIP conflict, DESIGN.md section 2n.  Node i is cost row 0 plus the
  * rows r >= 1 of the saved snapshot with keep[i * H + r] != 0 (H = the snapshot's height; row 0 is always kept), in
  * their original order, followed by the cut rows cuts[cut_offsets[i] .. cut_offsets[i+1]) appended as jslp_add_cuts

@@ -120,6 +120,7 @@ SYMBOLS = [
     ("jslp_column", C.c_int, [P, C.c_int, P]),
     ("jslp_pool_batch", C.c_int, [P, P, P, P, P, C.c_int, C.c_int, C.c_int, P, P, P, P, P, P, P, P]),
     ("jslp_target_batch", C.c_int, [P, P, P, P, P, C.c_int, C.c_int, C.c_int, P, P, P, P, P, P, P, P]),
+    ("jslp_box_batch", C.c_int, [P, P, P, P, P, C.c_int, C.c_int, C.c_int, P, P, P, P, P, P, P, P]),
     ("jslp_conflict_batch", C.c_int, [P, P, P, P, P, C.c_int, C.c_int, P, P, P, P, P, P, P]),
     ("jslp_branch_and_cut", C.c_int, [P, C.POINTER(BnbOpts), C.POINTER(BnbStatus), P, C.c_int]),
     ("jslp_bnb_batch", C.c_int, [P, P, P, C.c_int, C.POINTER(BnbOpts), C.c_int, P, P, P, P]),

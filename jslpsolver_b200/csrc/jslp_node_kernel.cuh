@@ -86,8 +86,9 @@ struct NodeBatchDev {
     // memory; every right-hand-side edit before every cost edit) to the restored root, solves, and writes its final
     // column 0 and row labels to out_rhs / out_vrow + n * Hcap (NODE_COLUMNS writes them too).  Not read by the other
     // modes.
-    // Pool launches (NODE_POOL: jslp_pool_batch, jslp_target_batch) apply edits[edit_off[n] .. edit_off[n+1]) (device
-    // memory) to the restored root: the EDIT_FIX_COL edits in list order, then, when cost_edits is set, the
+    // Pool launches (NODE_POOL: jslp_pool_batch, jslp_target_batch, jslp_box_batch) apply edits[edit_off[n] ..
+    // edit_off[n+1]) (device memory) to the restored root: the EDIT_RHS_COL / EDIT_RHS_ROW / EDIT_FIX_COL edits in list
+    // order as one row pass, then, when cost_edits is set, the
     // EDIT_COST_ROW / EDIT_COST_COL edits in list order as NODE_SCENARIO applies them; then they append node n's cut
     // rows as NODE_BRANCH does.  They write column 0 and the row labels too.  The final columns go to out_rhs /
     // out_vrow + n * Hcap.

@@ -8,24 +8,27 @@
 //
 // Regions whose rows fit shared memory run one CTA each in k_node_batch<NODE_POOL> (the fixings ride the scenario edit
 // loop as EDIT_FIX_COL edits); the others, and any region whose log shows a cycle or that hits the in-kernel pivot or
-// log cap, run one after another on the single-tableau path: jslp_restore, k_fix_columns, jslp_add_cuts, run_lp,
-// mip_scan.  Both apply the fixings with the same arithmetic in the same order.
+// log cap, run one after another on the single-tableau path: jslp_restore, k_row_edits, jslp_add_cuts, run_lp,
+// mip_scan.  Both apply the fixings with the same arithmetic in the same order.  jslp_target_batch (section 2o) adds
+// cost edits and jslp_box_batch (section 2s) right-hand-side edits to the same node LP.
 #pragma once
 
 namespace jslp {
 
-// The fixings of one region on the current buffer (the single-tableau path of jslp_pool_batch): one thread per row,
-// each fixing in list order, the arithmetic of k_node_batch<NODE_POOL>'s edit loop.
-__global__ void __launch_bounds__(256) k_fix_columns(const TabDev *Tp, const EditDev *fixes, int n) {
+// The row pass of one node on the current buffer (the single-tableau path of jslp_pool_batch, jslp_target_batch and
+// jslp_box_batch): one thread per row, the EDIT_RHS_COL, EDIT_RHS_ROW and EDIT_FIX_COL edits in list order, the
+// arithmetic of k_node_batch<NODE_POOL>'s row pass.  Other kinds are skipped: they belong to the column pass.
+__global__ void __launch_bounds__(256) k_row_edits(const TabDev *Tp, const EditDev *edits, int n) {
     const TabDev &T = *Tp;
     const int r = blockIdx.x * 256 + threadIdx.x;
     if (r >= T.H) return;
     double *row = T.M + (size_t)r * T.stride;
     double x = row[0];
     for (int k = 0; k < n; k++) {
-        const EditDev e = fixes[k];
-        x = edit_axpy_sub(x, e.d, row[e.pos]);
-        row[e.pos] = 0.0;
+        const EditDev e = edits[k];
+        if (e.kind == EDIT_RHS_COL) x = edit_axpy_sub(x, e.d, row[e.pos]);
+        else if (e.kind == EDIT_RHS_ROW && e.pos == r) x = edit_sub(x, e.d);
+        else if (e.kind == EDIT_FIX_COL) { x = edit_axpy_sub(x, e.d, row[e.pos]); row[e.pos] = 0.0; }
     }
     row[0] = x;
 }
@@ -51,22 +54,23 @@ struct PoolOut {
     }
 };
 
-// One node on the single-tableau path: the fixings by k_fix_columns, then the cost edits in list order with
-// jslp_update_cost's kernels (the arithmetic of k_node_batch<NODE_POOL>'s column pass), then the cut rows.  The caller
-// restores the snapshot.
+// One node on the single-tableau path: the right-hand-side edits and fixings by k_row_edits, then the cost edits in
+// list order with jslp_update_cost's kernels (the arithmetic of k_node_batch<NODE_POOL>'s column pass), then the cut
+// rows.  The caller restores the snapshot.
 static int pool_hbm(jslp_tab *t, const EditDev *edits, int n_edits, const jslp_cut *cuts, int n_cuts, int check_cycles,
                     int i, PoolOut &o) {
     cudaStream_t s = t->ctx->stream;
     int rc = jslp_restore(t);
     if (rc) return rc;
-    std::vector<EditDev> fixes;
+    std::vector<EditDev> rows;
     for (int k = 0; k < n_edits; k++)
-        if (edits[k].kind == EDIT_FIX_COL) fixes.push_back(edits[k]);
-    if (!fixes.empty()) {
-        rc = batch_scratch(t, sizeof(EditDev) * fixes.size());
+        if (edits[k].kind == EDIT_RHS_COL || edits[k].kind == EDIT_RHS_ROW || edits[k].kind == EDIT_FIX_COL)
+            rows.push_back(edits[k]);
+    if (!rows.empty()) {
+        rc = batch_scratch(t, sizeof(EditDev) * rows.size());
         if (rc) return rc;
-        CK(cudaMemcpyAsync(t->d_scratch, fixes.data(), sizeof(EditDev) * fixes.size(), cudaMemcpyHostToDevice, s));
-        k_fix_columns<<<(t->H + 255) / 256, 256, 0, s>>>(t->d_T, (const EditDev *)t->d_scratch, (int)fixes.size());
+        CK(cudaMemcpyAsync(t->d_scratch, rows.data(), sizeof(EditDev) * rows.size(), cudaMemcpyHostToDevice, s));
+        k_row_edits<<<(t->H + 255) / 256, 256, 0, s>>>(t->d_T, (const EditDev *)t->d_scratch, (int)rows.size());
         t->ctx->launches += 1;
         CK(cudaGetLastError());
     }
@@ -237,17 +241,11 @@ extern "C" int jslp_pool_batch(jslp_tab *t, const jslp_fix *fixes, const int32_t
     return pool_run(t, fx, fix_offsets, cuts, cut_offsets, n_nodes, check_cycles, o);
 }
 
-extern "C" int jslp_target_batch(jslp_tab *t, const jslp_scenario_edit *edits, const int32_t *edit_offsets,
-                                 const jslp_cut *cuts, const int32_t *cut_offsets, int n_nodes, int check_cycles,
-                                 int row_stride, int32_t *status, double *evaluation, int32_t *is_integral,
-                                 int32_t *branch_var, double *branch_value, int32_t *pivots, double *rhs, int32_t *vrow) {
-    int rc = pool_check(t, edit_offsets, cuts, cut_offsets, n_nodes, row_stride,
-                        status && evaluation && is_integral && branch_var && branch_value && pivots && rhs && vrow,
-                        "target_batch", "node");
-    if (rc || n_nodes == 0) return rc;
-    const int n_edits = edit_offsets[n_nodes], n_cuts = cut_offsets[n_nodes];
-    if ((n_edits > 0 && !edits) || (n_cuts > 0 && !cuts)) return fail(JSLP_E_INVALID, "target_batch: edits / cuts is NULL");
-    // updateCost resolved once against the snapshot's labels, as jslp_scenario_batch resolves it
+// The edits of jslp_target_batch and jslp_box_batch resolved once against the snapshot's labels, as
+// jslp_scenario_batch resolves them: kind 1 (updateCost) always, kind 0 (updateRightHandSide) when `rhs` is set, and
+// then only before the node's cost edits, so that the row pass and the column pass apply them in list order.
+static int node_edits(jslp_tab *t, const jslp_scenario_edit *edits, const int32_t *edit_offsets, int n_nodes, bool rhs,
+                      const std::string &what, std::vector<EditDev> &ed) {
     CK(cudaSetDevice(t->ctx->device));
     HostMaps m;
     m.vrow.resize((size_t)t->saved.H);
@@ -256,13 +254,52 @@ extern "C" int jslp_target_batch(jslp_tab *t, const jslp_scenario_edit *edits, c
     CK(cudaMemcpyAsync(m.vrow.data(), t->saved.vrow, sizeof(int) * m.vrow.size(), cudaMemcpyDeviceToHost, s));
     CK(cudaMemcpyAsync(m.vcol.data(), t->saved.vcol, sizeof(int) * m.vcol.size(), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
-    std::vector<EditDev> ed((size_t)n_edits);
-    for (int k = 0; k < n_edits; k++) {
-        if (edits[k].kind != 1) return fail(JSLP_E_INVALID, "target_batch: edit kind must be 1 (cost)");
-        if (!resolve_edit(m, edits[k], &ed[k])) return fail(JSLP_E_INVALID, "target_batch: unknown variable index");
-    }
-    rc = pool_check_cuts(t, cuts, n_cuts, "target_batch");
+    ed.resize((size_t)edit_offsets[n_nodes]);
+    for (int i = 0; i < n_nodes; i++)
+        for (int k = edit_offsets[i]; k < edit_offsets[i + 1]; k++) {
+            const int kind = edits[k].kind;
+            if (!rhs && kind != 1) return fail(JSLP_E_INVALID, what + ": edit kind must be 1 (cost)");
+            if (rhs && kind != 0 && kind != 1) return fail(JSLP_E_INVALID, what + ": edit kind must be 0 (rhs) or 1 (cost)");
+            if (kind == 0 && k > edit_offsets[i] && edits[k - 1].kind == 1)
+                return fail(JSLP_E_INVALID, what + ": a node's right-hand-side edits come before its cost edits");
+            if (!resolve_edit(m, edits[k], &ed[k]))
+                return fail(JSLP_E_INVALID, what + (rhs ? ": unknown constraint or variable index" : ": unknown variable index"));
+        }
+    return JSLP_OK;
+}
+
+// jslp_target_batch and jslp_box_batch: the checks, the edits resolved, the node LPs.
+static int edit_batch(jslp_tab *t, const jslp_scenario_edit *edits, const int32_t *edit_offsets, const jslp_cut *cuts,
+                      const int32_t *cut_offsets, int n_nodes, int check_cycles, int row_stride, int32_t *status,
+                      double *evaluation, int32_t *is_integral, int32_t *branch_var, double *branch_value,
+                      int32_t *pivots, double *rhs, int32_t *vrow, bool rhs_edits, const std::string &what) {
+    int rc = pool_check(t, edit_offsets, cuts, cut_offsets, n_nodes, row_stride,
+                        status && evaluation && is_integral && branch_var && branch_value && pivots && rhs && vrow,
+                        what, "node");
+    if (rc || n_nodes == 0) return rc;
+    const int n_edits = edit_offsets[n_nodes], n_cuts = cut_offsets[n_nodes];
+    if ((n_edits > 0 && !edits) || (n_cuts > 0 && !cuts)) return fail(JSLP_E_INVALID, what + ": edits / cuts is NULL");
+    std::vector<EditDev> ed;
+    rc = node_edits(t, edits, edit_offsets, n_nodes, rhs_edits, what, ed);
+    if (rc) return rc;
+    rc = pool_check_cuts(t, cuts, n_cuts, what);
     if (rc) return rc;
     PoolOut o{status, is_integral, branch_var, pivots, evaluation, branch_value, rhs, vrow, row_stride};
     return pool_run(t, ed, edit_offsets, cuts, cut_offsets, n_nodes, check_cycles, o);
+}
+
+extern "C" int jslp_target_batch(jslp_tab *t, const jslp_scenario_edit *edits, const int32_t *edit_offsets,
+                                 const jslp_cut *cuts, const int32_t *cut_offsets, int n_nodes, int check_cycles,
+                                 int row_stride, int32_t *status, double *evaluation, int32_t *is_integral,
+                                 int32_t *branch_var, double *branch_value, int32_t *pivots, double *rhs, int32_t *vrow) {
+    return edit_batch(t, edits, edit_offsets, cuts, cut_offsets, n_nodes, check_cycles, row_stride, status, evaluation,
+                      is_integral, branch_var, branch_value, pivots, rhs, vrow, false, "target_batch");
+}
+
+extern "C" int jslp_box_batch(jslp_tab *t, const jslp_scenario_edit *edits, const int32_t *edit_offsets,
+                              const jslp_cut *cuts, const int32_t *cut_offsets, int n_nodes, int check_cycles,
+                              int row_stride, int32_t *status, double *evaluation, int32_t *is_integral,
+                              int32_t *branch_var, double *branch_value, int32_t *pivots, double *rhs, int32_t *vrow) {
+    return edit_batch(t, edits, edit_offsets, cuts, cut_offsets, n_nodes, check_cycles, row_stride, status, evaluation,
+                      is_integral, branch_var, branch_value, pivots, rhs, vrow, true, "box_batch");
 }

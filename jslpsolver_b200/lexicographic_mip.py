@@ -108,17 +108,29 @@ def LexicographicMIP(solver, model: Any, gap=0.0, absolute_gap=0.0, max_nodes=10
 
     working = dict(model, optimize=keys[0], opType=senses[keys[0]])
     instance = solver._instance(working, precision)  # loadJson only: no presolve
+    tab = instance.tableau
+    try:
+        tab.setModel(instance)
+        out = chain(tab, instance, working, keys, senses, gaps, absolute, max_nodes, width, WHAT)
+    finally:
+        tab.close()
+    return out
+
+
+def chain(tab, instance, working: dict, keys, senses: dict, gaps, absolute, max_nodes: int, width: Optional[int],
+          what: str) -> dict:
+    """The levels of rules 1 and 2 over keys in order, from the initial tableau tab of `instance` (loaded from
+    `working`, whose objective is keys[0]; setModel done, no presolve), with allowances from gaps / absolute (one per
+    key).  Returns LexicographicMIP()'s result; every tableau derived from tab is closed, tab is not.
+    `what` names the caller in the refusal of a level-1 search that hits max_nodes before any integer plan."""
     n_ints = len(instance.initial_tableau().integerIndices)
     P = instance.precision
-    tab = instance.tableau
     levels: list = []
     out = {"feasible": True, "bounded": True, "stop": "reached", "objectives": None, "values": None,
            "levels": levels}
-    plan, cur, arg = None, None, 0.0
+    plan, cur, arg = None, tab, 0.0
+    launches0 = tab.context.launches
     try:
-        tab.setModel(instance)
-        launches0 = tab.context.launches
-        cur = tab
         for k, key in enumerate(keys):
             lv = level_entry(key, senses[key])
             levels.append(lv)
@@ -139,14 +151,14 @@ def LexicographicMIP(solver, model: Any, gap=0.0, absolute_gap=0.0, max_nodes=10
                     break
                 if state == "limit":
                     if best is None and plan is None:
-                        raise ValueError(f"{WHAT}: the search of level 1 ({key!r}) hit max_nodes={max_nodes} before "
+                        raise ValueError(f"{what}: the search of level 1 ({key!r}) hit max_nodes={max_nodes} before "
                                          "any integer plan; raise max_nodes")
                     lv["exact"], lv["bound"] = False, signed(senses[key], found["bound"])
                 if best is None and state == "exact":
                     if k == 0:  # no integer plan: Conflict() explains why
                         out["feasible"], out["stop"] = False, None
                         break
-                    raise RuntimeError(f"{WHAT}: level {k + 1} ({key!r}) has no integer plan, but the plan of level "
+                    raise RuntimeError(f"{what}: level {k + 1} ({key!r}) has no integer plan, but the plan of level "
                                        f"{k} is one")
                 if best is not None:
                     at = plan_values(best.rhs, best.vrow)
@@ -158,9 +170,9 @@ def LexicographicMIP(solver, model: Any, gap=0.0, absolute_gap=0.0, max_nodes=10
                     out["stop"] = "limit"
                     break
             if k + 1 < len(keys):
-                lv["allowance"] = t = allowance(key, gaps[k], absolute[k], lv["optimum"], WHAT)
+                lv["allowance"] = t = allowance(key, gaps[k], absolute[k], lv["optimum"], what)
                 if cur is not None:  # R_k and Delta_k
-                    d = delta(cur, lv, best, f"{WHAT}: the root LP of level {k + 1} ({key!r})")
+                    d = delta(cur, lv, best, f"{what}: the root LP of level {k + 1} ({key!r})")
                     if d is None:
                         out["stop"] = "cycled"
                         break
@@ -169,7 +181,6 @@ def LexicographicMIP(solver, model: Any, gap=0.0, absolute_gap=0.0, max_nodes=10
     finally:
         if cur is not None and cur is not tab:
             cur.close()
-        tab.close()
     if out["stop"] == "unbounded":
         out["bounded"] = False
     if plan is not None:

@@ -95,15 +95,17 @@ class _Search:
         return b
 
 
-def run(evaluate, targets, start: list, P: float, max_nodes: int, width: Optional[int], wave: int = 1) -> dict:
+def run(evaluate, targets, start: list, P: float, max_nodes: int, width: Optional[int], wave: int = 1,
+        shared: bool = True) -> dict:
     """The concurrent target searches of DESIGN.md section 2o (rules 4 to 8).  targets = [(label, sense, integer)];
     a label of None stands for the node LP's own objective, so its value at an integral node is the node's evaluation
     and its sense is -1 (the lexicographic levels of section 2q).  start[k] = target k's incumbent value at x*; a
     target without one starts at -s * math.inf (math.inf for a min target, such as the label-None target).
     evaluate([(k, cuts), ...]) -> [Node, ...], the nodes' LPs on the bound tableau with row 0 set to -s_k on label_k.
     Each round evaluates the children of the first `width` open nodes (None: wave // live searches, at least 1) of
-    every live search in one call, then commits the searches in target order.  Returns {"best", "witness" (Node or
-    None: x*), "state", "bound", "nodes", "lps", "rounds"}."""
+    every live search in one call, then commits the searches in target order.  With shared=False an integral plan is
+    an incumbent of its own search only (the searches of section 2s run on different feasible regions).  Returns
+    {"best", "witness" (Node or None: x*), "state", "bound", "nodes", "lps", "rounds"}."""
     n = len(targets)
     searches = [_Search(k, lab, s, integer) for k, (lab, s, integer) in enumerate(targets)]
     best, witness = list(start), [None] * n
@@ -111,9 +113,9 @@ def run(evaluate, targets, start: list, P: float, max_nodes: int, width: Optiona
     def beats(sr: _Search, value: float) -> bool:
         return sr.s * (value - best[sr.k]) > P
 
-    def share(node: Node) -> None:
+    def share(node: Node, owner: _Search) -> None:
         at = plan_values(node.rhs, node.vrow)
-        for sr in searches:
+        for sr in searches if shared else [owner]:
             v = node.evaluation if sr.label is None else at.get(sr.label, 0.0)
             if beats(sr, v):
                 best[sr.k], witness[sr.k] = v, node
@@ -132,7 +134,7 @@ def run(evaluate, targets, start: list, P: float, max_nodes: int, width: Optiona
                 return
             heapq.heappop(sr.heap)
             if top.integral:
-                share(top)
+                share(top, sr)
                 continue
             sr.nodes += len(top.children)
             for c in top.children:

@@ -7,6 +7,7 @@ from typing import Any, Optional
 from . import validation
 from .conflict import Conflict as _conflict
 from .frontier import Frontier as _frontier
+from .frontier_mip import FrontierMIP as _frontier_mip
 from .lexicographic import Lexicographic as _lexicographic
 from .lexicographic_mip import LexicographicMIP as _lexicographic_mip
 from .mip_scenarios import Scenarios as _scenarios
@@ -70,6 +71,14 @@ class Solver:
         """The Pareto frontier of a continuous LP with exactly two objectives: every efficient vertex from the first
         objective's optimum to the second's, with the weights that select it (frontier.py, DESIGN.md section 2g)."""
         return _frontier(self, model, precision, validate)
+
+    def FrontierMIP(self, model: dict, *, step=None, max_points=1000, max_nodes=10000, width=None,
+                    precision: Optional[float] = None, validate: bool = False) -> dict:
+        """The Pareto frontier of a MIP with exactly two objectives: every nondominated image over the integer plans,
+        from the first objective's lexicographic optimum to the second's, each box of the balanced box method searched
+        exactly (frontier_mip.py, DESIGN.md section 2s).  `width` tunes the batching only."""
+        return _frontier_mip(self, model, step=step, max_points=max_points, max_nodes=max_nodes, width=width,
+                             precision=precision, validate=validate)
 
     def Lexicographic(self, model: dict, gap=0.0, absolute_gap=0.0, precision: Optional[float] = None,
                       validate: bool = False) -> dict:
@@ -178,6 +187,12 @@ def Solve(model: Any, precision: Optional[float] = None, full: bool = False, val
 
 def Frontier(model: dict, precision: Optional[float] = None, validate: bool = False) -> dict:
     return solver.Frontier(model, precision, validate)
+
+
+def FrontierMIP(model: dict, *, step=None, max_points=1000, max_nodes=10000, width=None,
+                precision: Optional[float] = None, validate: bool = False) -> dict:
+    return solver.FrontierMIP(model, step=step, max_points=max_points, max_nodes=max_nodes, width=width,
+                              precision=precision, validate=validate)
 
 
 def Lexicographic(model: dict, gap=0.0, absolute_gap=0.0, precision: Optional[float] = None,

@@ -882,17 +882,29 @@ class GpuTableau:
         section 2o).  nodes = [(edits, cuts), ...] with edits [(1, label, difference), ...] applied in order to the
         saved snapshot as updateCost applies them, then the cuts appended and simplex() run as pool_batch does.
         Returns what pool_batch returns.  Leaves the tableau equal to its snapshot."""
+        return self._node_batch(self.context.lib.jslp_target_batch, self._edit_array(nodes), nodes, check_cycles)
+
+    def box_batch(self, nodes, check_cycles: Optional[bool] = None) -> dict:
+        """jslp_box_batch: the node LPs of the box searches of a two-objective MIP's frontier (DESIGN.md section 2s).
+        nodes = [(edits, cuts), ...] with edits [(kind, label, difference), ...] -- kind 0 = updateRightHandSide, before
+        any kind 1 = updateCost -- applied in order to the saved snapshot, then the cuts appended and simplex() run as
+        pool_batch does.  Returns what pool_batch returns.  Leaves the tableau equal to its snapshot."""
+        return self._node_batch(self.context.lib.jslp_box_batch, self._edit_array(nodes), nodes, check_cycles)
+
+    @staticmethod
+    def _edit_array(nodes):
+        """The edits of nodes = [(edits of node i, cuts of node i), ...] as one ctypes array, in node order."""
         arr = (ScenarioEdit * max(1, sum(len(ed) for ed, _ in nodes)))()
         k = 0
         for ed, _ in nodes:
             for kind, index, difference in ed:
                 arr[k].kind, arr[k].index, arr[k].difference = int(kind), int(index), float(difference)
                 k += 1
-        return self._node_batch(self.context.lib.jslp_target_batch, arr, nodes, check_cycles)
+        return arr
 
     def _node_batch(self, fn, edits, nodes, check_cycles: Optional[bool]) -> dict:
-        """The call and outputs jslp_pool_batch and jslp_target_batch share: edits (a ctypes array) in the order of
-        nodes = [(edits of node i, cuts of node i), ...]."""
+        """The call and outputs jslp_pool_batch, jslp_target_batch and jslp_box_batch share: edits (a ctypes array) in
+        the order of nodes = [(edits of node i, cuts of node i), ...]."""
         n = len(nodes)
         edit_off, cut_off = np.zeros(n + 1, dtype=np.int32), np.zeros(n + 1, dtype=np.int32)
         for i, (ed, cs) in enumerate(nodes):
