@@ -517,6 +517,28 @@ typedef struct {
 
 int jslp_branch_and_cut(jslp_tab *root, const jslp_bnb_opts *opts, jslp_bnb_status *out,
                         jslp_cut *best_cuts, int best_cuts_cap);
+/* MIP starts, DESIGN.md section 2t: jslp_branch_and_cut (default service) seeded with known integer plans.  Start i is
+ * the cut list start_cuts[start_offsets[i] .. start_offsets[i + 1]) on integer labels.  Right after the root is
+ * committed fractional (where the snapshot is taken), each start's node is evaluated from the snapshot as every node
+ * is; a feasible fractional node begins a depth-first dive (most fractional variable, nearer child first) of at most
+ * start_nodes node LPs, all live dives advancing together, one node batch per wave.  The integral node with the
+ * smallest evaluation (lowest index on a tie) becomes the incumbent before the next pop, without an iteration or a
+ * node-log entry; the loop then runs unchanged.  iterations, nodes_evaluated, pivots, max_nodes and the node log count
+ * tree nodes only; kernel_launches counts the whole call.  The tableau and its scalar state leave the seed stage as
+ * the root left them.  n_starts = 0 is jslp_branch_and_cut.  With n_starts > 0, opts->service != 0, n_ranks > 1 and
+ * optional objectives are JSLP_E_UNSUPPORTED.                                                                        */
+enum { JSLP_START_SEED = 0, JSLP_START_FEASIBLE = 1, JSLP_START_INFEASIBLE = 2, JSLP_START_INCOMPLETE = 3,
+       JSLP_START_SKIPPED = 4 };
+typedef struct {
+    int32_t status;    /* JSLP_START_*: skipped when the root was integral, infeasible or unbounded        */
+    int32_t n_cuts;    /* cuts of its integral node (0 when none)                                          */
+    int64_t nodes;     /* node LPs of its dive                                                             */
+    int64_t pivots;    /* pivots of those node LPs                                                         */
+    double evaluation; /* of its integral node (Tableau.evaluation, minimisation sense); NaN when none    */
+} jslp_start_status;
+int jslp_branch_and_cut_start(jslp_tab *root, const jslp_bnb_opts *opts, const jslp_cut *start_cuts,
+                              const int32_t *start_offsets, int n_starts, int64_t start_nodes,
+                              jslp_start_status *starts, jslp_bnb_status *out, jslp_cut *best_cuts, int best_cuts_cap);
 /* What-if scenarios of a MIP, DESIGN.md section 2p: scenario s is jslp_branch_and_cut's default service (service 0)
  * over the tab's current tableau with rows 1.. of column 0 replaced by col0[s * H + r] and row 0 by row0[s * W + c]
  * (H x W = the tab's size), every tree committed in its own best-first order.  Each round evaluates the next

@@ -62,6 +62,14 @@ class BnbStatus(C.Structure):
         ("collectives", C.c_int64), ("slot_pivots", C.c_int64), ("slot_ms", C.c_double), ("slot_bytes", C.c_double)]
 
 
+class StartStatus(C.Structure):  # jslp_start_status
+    _fields_ = [("status", C.c_int32), ("n_cuts", C.c_int32), ("nodes", C.c_int64), ("pivots", C.c_int64),
+                ("evaluation", C.c_double)]
+
+
+START_SEED, START_FEASIBLE, START_INFEASIBLE, START_INCOMPLETE, START_SKIPPED = 0, 1, 2, 3, 4
+
+
 # every symbol include/jslp_b200.h declares: (name, restype, argtypes)
 P = C.c_void_p
 SYMBOLS = [
@@ -123,6 +131,8 @@ SYMBOLS = [
     ("jslp_box_batch", C.c_int, [P, P, P, P, P, C.c_int, C.c_int, C.c_int, P, P, P, P, P, P, P, P]),
     ("jslp_conflict_batch", C.c_int, [P, P, P, P, P, C.c_int, C.c_int, P, P, P, P, P, P, P]),
     ("jslp_branch_and_cut", C.c_int, [P, C.POINTER(BnbOpts), C.POINTER(BnbStatus), P, C.c_int]),
+    ("jslp_branch_and_cut_start", C.c_int, [P, C.POINTER(BnbOpts), P, P, C.c_int, C.c_int64, P,
+                                            C.POINTER(BnbStatus), P, C.c_int]),
     ("jslp_bnb_batch", C.c_int, [P, P, P, C.c_int, C.POINTER(BnbOpts), C.c_int, P, P, P, P]),
     ("jslp_bnb_node_log", C.c_int, [P, P, C.c_int64, C.POINTER(C.c_int64)]),
     ("jslp_bnb_solution", C.c_int, [P, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_int32), P, P, C.c_int]),

@@ -397,8 +397,18 @@ static int eval_nodes_resident(jslp_tab *t, jslp_bnb::Branch *const *nodes, int 
     return JSLP_OK;
 }
 
-extern "C" int jslp_branch_and_cut(jslp_tab *t, const jslp_bnb_opts *opts, jslp_bnb_status *out,
-                                   jslp_cut *best_cuts, int best_cuts_cap) {
+// The starts of jslp_branch_and_cut_start (DESIGN.md section 2t): start i is cuts[off[i] .. off[i + 1]).
+struct StartSet {
+    const jslp_cut *cuts;
+    const int32_t *off;
+    int n;
+    int64_t max_nodes;
+    jslp_start_status *st;
+};
+
+// jslp_branch_and_cut, seeded by the starts of ss when it is set.
+static int branch_and_cut(jslp_tab *t, const jslp_bnb_opts *opts, const StartSet *ss, jslp_bnb_status *out,
+                          jslp_cut *best_cuts, int best_cuts_cap) {
     using namespace jslp_bnb;
     if (!t || !opts) return fail(JSLP_E_INVALID, "NULL argument");
     if (t->n_int <= 0) return fail(JSLP_E_INVALID, "branch_and_cut needs integer variables (upload int_var_indices)");
@@ -463,6 +473,128 @@ extern "C" int jslp_branch_and_cut(jslp_tab *t, const jslp_bnb_opts *opts, jslp_
         t->bestPossibleEval = tree.bestPossibleEval; t->simplexIters = tree.simplexIters; t->isIntegralFlag = tree.isIntegral;
     };
 
+    // One round's node LPs, todo in pop order, on the path their heights and the options choose: shared-memory node
+    // batch, node slots or one after another on the single-tableau path, sharded over the ranks as the options ask.  U
+    // is the round's incumbent bound (see eval_nodes_slots); count gains this rank's node LPs.
+    auto eval_round = [&](std::vector<Branch *> &todo, double &U, int64_t &count) -> int {
+        int maxc_all = 0;
+        for (Branch *b : todo) maxc_all = std::max(maxc_all, (int)b->cuts.size());
+        // every rank takes the same decisions from the same (rank-independent) quantities
+        // useMIRCuts: the MIR loop (fractional volume, cut rows, re-solves) runs on the single-tableau path
+        const bool resident = iterations > 0 && t->saved.valid && t->engine != 1 && t->engine != 2 && !t->use_mir &&
+                              resident_fits(t, t->saved.H + maxc_all);
+        const int nslots = (!resident && !t->use_mir && iterations > 0 && t->saved.valid && todo.size() >= 2)
+                               ? slots_for(t, t->saved.H + maxc_all, std::max(K, (int)todo.size())) : 0;
+        // The root round is NOT sharded: every rank needs the solved root in its own tableau, it is what
+        // jslp_save snapshots and what every later node is derived from.  Rounds of nodes that fit shared
+        // memory are not sharded either unless asked: a whole round costs less than one collective.
+        const bool sharded = n_ranks > 1 && iterations > 0 && !t->use_mir && (opts->shard_policy == 1 || !resident);
+        std::vector<Branch *> mine;
+        for (size_t i = 0; i < todo.size(); i++)
+            if (!sharded || (int)(i % n_ranks) == rank) mine.push_back(todo[i]);
+        if (resident) {
+            if (!mine.empty()) {
+                int rc = eval_nodes_resident(t, mine.data(), (int)mine.size(), check_cycles);
+                if (rc) return rc;
+            }
+        } else if (nslots >= 2) {
+            int rc = eval_nodes_slots(t, mine.data(), (int)mine.size(), nslots, check_cycles, &U, sharded ? &ex : nullptr, &pruned);
+            if (rc) return rc;
+        } else {
+            for (Branch *b : mine) {
+                if (b->relaxedEvaluation > U) { pruned++; continue; }
+                int rc = eval_node_streaming(t, *b, check_cycles, b->ev);
+                if (rc) return rc;
+                if (b->ev.feasible && b->ev.is_integral && b->ev.evaluation < U) U = b->ev.evaluation;
+            }
+        }
+        count += (int64_t)mine.size();
+        if (sharded) {  // all-gather the summaries: rank-major blocks of `per` records
+            const int per = (int)((todo.size() + n_ranks - 1) / n_ranks);
+            wire.assign((size_t)per * n_ranks * WIRE_DOUBLES, 0.0);
+            for (size_t j = 0; j < mine.size(); j++)
+                to_wire(mine[j]->ev, &wire[((size_t)rank * per + j) * WIRE_DOUBLES]);
+            int rc = ex.gather(wire.data(), (int64_t)per * WIRE_DOUBLES * 8);
+            if (rc) return rc;
+            for (size_t i = 0; i < todo.size(); i++)
+                from_wire(todo[i]->ev, &wire[((size_t)(i % n_ranks) * per + i / n_ranks) * WIRE_DOUBLES]);
+        }
+        return JSLP_OK;
+    };
+
+    // The seed stage (DESIGN.md section 2t), run where the root was committed fractional and snapshotted: every
+    // start's node from the snapshot, then depth-first dives from the feasible fractional ones, one node of every live
+    // dive per wave, each wave one eval_round.  The best integral node becomes the incumbent; the tableau and the
+    // tab's scalar state are then put back as the root left them.
+    auto seed_stage = [&]() -> int {
+        struct Dive {
+            std::vector<std::unique_ptr<Branch>> stack;  // top = back
+            std::unique_ptr<Branch> found;
+            bool live = true;
+        };
+        std::vector<Dive> dives((size_t)ss->n);
+        for (int i = 0; i < ss->n; i++) {
+            dives[i].stack.emplace_back(new Branch{
+                -INFINITY, std::vector<jslp_cut>(ss->cuts + ss->off[i], ss->cuts + ss->off[i + 1]), NodeEval()});
+            ss->st[i].status = JSLP_START_INFEASIBLE;
+        }
+        for (;;) {
+            std::vector<Branch *> wave;
+            std::vector<int> who;
+            for (int i = 0; i < ss->n; i++) {
+                Dive &d = dives[i];
+                if (!d.live) continue;
+                if (d.stack.empty()) { d.live = false; continue; }
+                if (ss->st[i].nodes >= ss->max_nodes) { ss->st[i].status = JSLP_START_INCOMPLETE; d.live = false; continue; }
+                wave.push_back(d.stack.back().get());
+                who.push_back(i);
+            }
+            if (wave.empty()) break;
+            double U = INFINITY;  // a start node sorts before nothing: none is dropped
+            int64_t count = 0;
+            int rc = eval_round(wave, U, count);
+            if (rc) return rc;
+            for (int i : who) {
+                Dive &d = dives[i];
+                jslp_start_status &st = ss->st[i];
+                std::unique_ptr<Branch> b = std::move(d.stack.back());
+                d.stack.pop_back();
+                const NodeEval ev = b->ev;
+                st.nodes++;
+                st.pivots += ev.pivots;
+                if (!ev.feasible) continue;
+                if (ev.is_integral) {
+                    st.status = JSLP_START_FEASIBLE;
+                    st.evaluation = ev.evaluation;
+                    st.n_cuts = (int)b->cuts.size();
+                    d.found = std::move(b);
+                    d.live = false;
+                    continue;
+                }
+                std::unique_ptr<Branch> high, low;
+                Tree::children(*b, ev.branch_var, ev.branch_value, -INFINITY, high, low);
+                const bool up = ev.branch_value - std::floor(ev.branch_value) >= 0.5;  // the nearer child on top
+                d.stack.push_back(std::move(up ? low : high));
+                d.stack.push_back(std::move(up ? high : low));
+            }
+        }
+        int best = -1;
+        for (int i = 0; i < ss->n; i++)
+            if (dives[i].found && (best < 0 || ss->st[i].evaluation < ss->st[best].evaluation)) best = i;
+        if (best >= 0) {
+            ss->st[best].status = JSLP_START_SEED;
+            tree.seed(std::move(dives[best].found->cuts), ss->st[best].evaluation);
+            if (opts->keep_solutions) {
+                int rc = store_solution(*tree.bestBranch);
+                if (rc) return rc;
+            }
+        }
+        int rc = jslp_restore(t);
+        if (rc) return rc;
+        store();
+        return JSLP_OK;
+    };
+
     double eval_ms = 0, commit_ms = 0, root_ms = 0, final_ms = 0;
     t->node_kernel_ns = 0;
     bool stop = false;
@@ -475,48 +607,8 @@ extern "C" int jslp_branch_and_cut(jslp_tab *t, const jslp_bnb_opts *opts, jslp_
         const auto t_eval = now();
         if (!todo.empty()) {
             rounds++;
-            int maxc_all = 0;
-            for (Branch *b : todo) maxc_all = std::max(maxc_all, (int)b->cuts.size());
-            // every rank takes the same decisions from the same (rank-independent) quantities
-            // useMIRCuts: the MIR loop (fractional volume, cut rows, re-solves) runs on the single-tableau path
-            const bool resident = iterations > 0 && t->saved.valid && t->engine != 1 && t->engine != 2 && !t->use_mir &&
-                                  resident_fits(t, t->saved.H + maxc_all);
-            const int nslots = (!resident && !t->use_mir && iterations > 0 && t->saved.valid && todo.size() >= 2)
-                                   ? slots_for(t, t->saved.H + maxc_all, std::max(K, (int)todo.size())) : 0;
-            // The root round is NOT sharded: every rank needs the solved root in its own tableau, it is what
-            // jslp_save snapshots and what every later node is derived from.  Rounds of nodes that fit shared
-            // memory are not sharded either unless asked: a whole round costs less than one collective.
-            const bool sharded = n_ranks > 1 && iterations > 0 && !t->use_mir && (opts->shard_policy == 1 || !resident);
-            std::vector<Branch *> mine;
-            for (size_t i = 0; i < todo.size(); i++)
-                if (!sharded || (int)(i % n_ranks) == rank) mine.push_back(todo[i]);
-            if (resident) {
-                if (!mine.empty()) {
-                    int rc = eval_nodes_resident(t, mine.data(), (int)mine.size(), check_cycles);
-                    if (rc) return rc;
-                }
-            } else if (nslots >= 2) {
-                int rc = eval_nodes_slots(t, mine.data(), (int)mine.size(), nslots, check_cycles, &U, sharded ? &ex : nullptr, &pruned);
-                if (rc) return rc;
-            } else {
-                for (Branch *b : mine) {
-                    if (b->relaxedEvaluation > U) { pruned++; continue; }
-                    int rc = eval_node_streaming(t, *b, check_cycles, b->ev);
-                    if (rc) return rc;
-                    if (b->ev.feasible && b->ev.is_integral && b->ev.evaluation < U) U = b->ev.evaluation;
-                }
-            }
-            nodes += (int64_t)mine.size();
-            if (sharded) {  // all-gather the summaries: rank-major blocks of `per` records
-                const int per = (int)((todo.size() + n_ranks - 1) / n_ranks);
-                wire.assign((size_t)per * n_ranks * WIRE_DOUBLES, 0.0);
-                for (size_t j = 0; j < mine.size(); j++)
-                    to_wire(mine[j]->ev, &wire[((size_t)rank * per + j) * WIRE_DOUBLES]);
-                int rc = ex.gather(wire.data(), (int64_t)per * WIRE_DOUBLES * 8);
-                if (rc) return rc;
-                for (size_t i = 0; i < todo.size(); i++)
-                    from_wire(todo[i]->ev, &wire[((size_t)(i % n_ranks) * per + i / n_ranks) * WIRE_DOUBLES]);
-            }
+            int rc = eval_round(todo, U, nodes);
+            if (rc) return rc;
         }
         tree.put_back(taken);
         if (iterations == 0) root_ms += ms_since(t_eval);
@@ -545,6 +637,10 @@ extern "C" int jslp_branch_and_cut(jslp_tab *t, const jslp_bnb_opts *opts, jslp_
             if (st == Tree::SNAPSHOT) {  // snapshot = optimal root tableau (branch-and-cut.ts:155-157)
                 int rc = jslp_save(t);
                 if (rc) return rc;
+                if (ss && tree.bounded) {
+                    rc = seed_stage();
+                    if (rc) return rc;
+                }
             } else if (st == Tree::INCUMBENT && opts->keep_solutions) {
                 int rc = store_solution(*tree.lastCommitted);
                 if (rc) return rc;
@@ -596,6 +692,36 @@ extern "C" int jslp_branch_and_cut(jslp_tab *t, const jslp_bnb_opts *opts, jslp_
         out->slot_pivots = t->slot_pivots; out->slot_ms = t->slot_ms; out->slot_bytes = t->slot_bytes;
     }
     return JSLP_OK;
+}
+
+extern "C" int jslp_branch_and_cut(jslp_tab *t, const jslp_bnb_opts *opts, jslp_bnb_status *out,
+                                   jslp_cut *best_cuts, int best_cuts_cap) {
+    return branch_and_cut(t, opts, nullptr, out, best_cuts, best_cuts_cap);
+}
+
+extern "C" int jslp_branch_and_cut_start(jslp_tab *t, const jslp_bnb_opts *opts, const jslp_cut *start_cuts,
+                                         const int32_t *start_offsets, int n_starts, int64_t start_nodes,
+                                         jslp_start_status *starts, jslp_bnb_status *out, jslp_cut *best_cuts,
+                                         int best_cuts_cap) {
+    if (n_starts == 0) return branch_and_cut(t, opts, nullptr, out, best_cuts, best_cuts_cap);
+    if (!t || !opts) return fail(JSLP_E_INVALID, "NULL argument");
+    if (n_starts < 0 || !start_offsets || !starts) return fail(JSLP_E_INVALID, "branch_and_cut_start: bad starts / offsets / status arguments");
+    if (start_nodes < 1) return fail(JSLP_E_INVALID, "branch_and_cut_start: start_nodes must be at least 1");
+    if (opts->service != 0) return fail(JSLP_E_UNSUPPORTED, "branch_and_cut_start: MIP starts need the default branch-and-cut service");
+    if (opts->n_ranks > 1) return fail(JSLP_E_UNSUPPORTED, "branch_and_cut_start: MIP starts run on one GPU (n_ranks must be 1)");
+    if (t->nOpt > 0) return fail(JSLP_E_UNSUPPORTED, "branch_and_cut_start: optional objectives are not supported");
+    int rc = batch_check_offsets({start_offsets}, n_starts, "branch_and_cut_start", "start_offsets[0]");
+    if (rc) return rc;
+    if (start_offsets[n_starts] > 0 && !start_cuts) return fail(JSLP_E_INVALID, "branch_and_cut_start: start_cuts is NULL");
+    for (int k = 0; k < start_offsets[n_starts]; k++) {
+        const int v = start_cuts[k].var_index;
+        if ((start_cuts[k].type != 0 && start_cuts[k].type != 1) || v < 0 || v >= (int)t->h_intpos.size() ||
+            t->h_intpos[v] < 0)
+            return fail(JSLP_E_INVALID, "branch_and_cut_start: a start cut is type 0 (min) or 1 (max) on an integer label");
+    }
+    for (int i = 0; i < n_starts; i++) starts[i] = jslp_start_status{JSLP_START_SKIPPED, 0, 0, 0, NAN};
+    const StartSet ss{start_cuts, start_offsets, n_starts, start_nodes, starts};
+    return branch_and_cut(t, opts, &ss, out, best_cuts, best_cuts_cap);
 }
 
 extern "C" int jslp_bnb_solution(jslp_tab *t, int i, double *evaluation, int32_t *height, int32_t *vrow, double *rhs, int cap) {

@@ -167,6 +167,32 @@ struct Tree {
         taken.clear();
     }
 
+    // A known integral plan as the incumbent (MIP starts, DESIGN.md section 2t): it is not a node of the loop, so it
+    // counts no iteration and writes no node-log entry.
+    void seed(std::vector<jslp_cut> cuts, double eval) {
+        bestEvaluation = eval;
+        isIntegral = 1;
+        bestBranch.reset(new Branch{eval, std::move(cuts), NodeEval()});
+    }
+
+    // The two children of a fractional node (branch-and-cut.ts:166-188): a cut on the branching variable goes to low
+    // when it is a `min` cut and to high when it is a `max` cut, every other cut to both, then each child's new cut.
+    static void children(const Branch &b, int varIndex, double value, double relaxed, std::unique_ptr<Branch> &high,
+                         std::unique_ptr<Branch> &low) {
+        high.reset(new Branch{relaxed, {}, NodeEval()});
+        low.reset(new Branch{relaxed, {}, NodeEval()});
+        for (const jslp_cut &cut : b.cuts) {
+            if (cut.var_index == varIndex) {
+                if (cut.type == 0) low->cuts.push_back(cut); else high->cuts.push_back(cut);
+            } else {
+                high->cuts.push_back(cut);
+                low->cuts.push_back(cut);
+            }
+        }
+        high->cuts.push_back(jslp_cut{0, varIndex, std::ceil(value)});
+        low->cuts.push_back(jslp_cut{1, varIndex, std::floor(value)});
+    }
+
     // The node the reference re-solves once the loop ends (branch-and-cut.ts:195-197): the incumbent, else the last
     // committed node when more than one was committed; null after the early return at an integral root.
     const Branch *final_branch() const {
@@ -216,17 +242,8 @@ struct Tree {
         }
         const int varIndex = ev.branch_var;
         nl.v[4] = 0; nl.v[5] = varIndex; nl.v[6] = ev.branch_value;
-        std::unique_ptr<Branch> high(new Branch{value, {}, NodeEval()}), low(new Branch{value, {}, NodeEval()});
-        for (const jslp_cut &cut : active->cuts) {  // branch-and-cut.ts:166-179
-            if (cut.var_index == varIndex) {
-                if (cut.type == 0) low->cuts.push_back(cut); else high->cuts.push_back(cut);
-            } else {
-                high->cuts.push_back(cut);
-                low->cuts.push_back(cut);
-            }
-        }
-        high->cuts.push_back(jslp_cut{0, varIndex, std::ceil(ev.branch_value)});
-        low->cuts.push_back(jslp_cut{1, varIndex, std::floor(ev.branch_value)});
+        std::unique_ptr<Branch> high, low;
+        children(*active, varIndex, ev.branch_value, value, high, low);
         branches.push(std::move(high));
         branches.push(std::move(low));
         const bool root = iterations == 1;

@@ -428,10 +428,16 @@ class Model:
         return InitialTableau(M, vrow, vcol, unres, ints, prios, costs)
 
     # ------------------------------------------------------------------ solve (model.ts:427-467)
-    def solve(self, *, basis=None):
+    def solve(self, *, basis=None, start=None, start_nodes: int = 1000):
         if basis is not None:  # warm start from a saved basis (DESIGN.md section 2f)
+            if start is not None:
+                from .mipstart import check_json
+                check_json({}, basis)
             from .warmstart import solve
             return solve(self, basis)
+        if start is not None:  # MIP starts (DESIGN.md section 2t)
+            from .mipstart import solve
+            return solve(self, start, start_nodes)
         if self.usePresolve and self.presolveResult is None:
             self.presolveResult = presolve(self)
             if self.presolveResult.isInfeasible:

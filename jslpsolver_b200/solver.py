@@ -31,7 +31,12 @@ class Solver:
         self.options: dict = {}    # JSLP_OPT_* -> value for every tableau this solver creates (tuning / test aids)
 
     def Solve(self, model: Any, precision: Optional[float] = None, full: bool = False, validate: bool = False, *,
-              basis: Optional[dict] = None):
+              basis: Optional[dict] = None, start=None, start_nodes: int = 1000):
+        """main.ts Solve.  `basis` warm-starts a continuous LP (DESIGN.md section 2f); `start`, a {variable: value}
+        plan or a list of them, seeds the branch and cut of a MIP with at most `start_nodes` node LPs per start to
+        complete each (DESIGN.md section 2t), reported under Solution.mipStart with full=True."""
+        if start is not None:
+            return self._solve_start(model, precision, full, validate, basis, start, start_nodes)
         if basis is not None:  # warm start from a saved basis (DESIGN.md section 2f)
             return self._solve_warm(model, precision, full, validate, basis)
         if validate:
@@ -62,6 +67,21 @@ class Solver:
                 raise NotImplementedError("external solvers (src/external) are out of scope")
         instance = self._instance(model, precision)
         solution = instance.solve(basis=basis)
+        return self._finish(instance, solution, full)
+
+    def _solve_start(self, model: Any, precision: Optional[float], full: bool, validate: bool, basis, start,
+                     start_nodes: int):
+        from .mipstart import check_json
+        if validate:
+            model = validation.validate(model)
+        if not model:
+            raise ValueError("Solver requires a model to operate on")
+        if isinstance(model, dict):
+            check_json(model, basis)
+        elif basis is not None:
+            check_json({}, basis)
+        instance = self._instance(model, precision)
+        solution = instance.solve(start=start, start_nodes=start_nodes)
         return self._finish(instance, solution, full)
 
     def MultiObjective(self, model: dict):  # main.ts:209-211
@@ -181,8 +201,8 @@ solver = Solver()
 
 
 def Solve(model: Any, precision: Optional[float] = None, full: bool = False, validate: bool = False, *,
-          basis: Optional[dict] = None):
-    return solver.Solve(model, precision, full, validate, basis=basis)
+          basis: Optional[dict] = None, start=None, start_nodes: int = 1000):
+    return solver.Solve(model, precision, full, validate, basis=basis, start=start, start_nodes=start_nodes)
 
 
 def Frontier(model: dict, precision: Optional[float] = None, validate: bool = False) -> dict:

@@ -20,7 +20,7 @@ from typing import Optional
 import numpy as np
 
 from . import _lib
-from ._lib import BnbOpts, BnbStatus, Cut, JslpError, LpStatus, ScenarioEdit
+from ._lib import BnbOpts, BnbStatus, Cut, JslpError, LpStatus, ScenarioEdit, StartStatus
 
 EPSILON = 2.220446049250313e-16
 
@@ -483,7 +483,10 @@ class GpuTableau:
         _lib.check(self.context.lib.jslp_most_fractional(self._h(), C.byref(i), C.byref(v)))
         return {"index": None if i.value < 0 else i.value, "value": v.value}
 
-    def branchAndCut(self) -> None:  # tableau.ts:244-246
+    def branchAndCut(self, start=None, start_nodes: int = 1000) -> None:  # tableau.ts:244-246
+        """Branch and cut of the tableau; `start` (DESIGN.md section 2t) is a list of MIP starts, each a list of
+        (type, varIndex, value) cuts on integer labels, seeding the incumbent through jslp_branch_and_cut_start, with
+        at most `start_nodes` node LPs per start.  Their outcomes go to lastStartStatus."""
         if self.branchAndCutService is not None:
             self.branchAndCutService.branchAndCut(self)
             return
@@ -520,9 +523,20 @@ class GpuTableau:
         if self.slot_steps is not None:
             self.set_option(_lib.OPT_SLOT_STEPS, self.slot_steps)
         st = BnbStatus()
-        cap = 4096
+        # a cut list holds at most one min and one max cut per integer variable
+        cap = max(4096, 2 * getattr(self, "nInts", 0))
         best = (Cut * cap)()
-        _lib.check(self.context.lib.jslp_branch_and_cut(self._h(), C.byref(opts), C.byref(st), best, cap))
+        if start is None:
+            _lib.check(self.context.lib.jslp_branch_and_cut(self._h(), C.byref(opts), C.byref(st), best, cap))
+        else:
+            offsets = np.zeros(len(start) + 1, dtype=np.int32)
+            offsets[1:] = np.cumsum([len(c) for c in start])
+            cuts = self._cut_array([c for cl in start for c in cl])
+            status = (StartStatus * max(1, len(start)))()
+            _lib.check(self.context.lib.jslp_branch_and_cut_start(self._h(), C.byref(opts), cuts, offsets.ctypes.data,
+                                                                  len(start), int(start_nodes), status, C.byref(st),
+                                                                  best, cap))
+            self.lastStartStatus = [status[i] for i in range(len(start))]
         self.lastBnbStatus = st
         self.feasible, self.bounded = bool(st.feasible), bool(st.bounded)
         self.evaluation, self.bestPossibleEval = st.evaluation, st.best_possible_eval
@@ -998,9 +1012,9 @@ class GpuTableau:
             r = row_of[var.index] if var.index < len(row_of) else -1
             var.value = 0 if r == -1 else js_round((float(rhs[r]) + EPSILON) * rounding) / rounding
 
-    def solve(self):
+    def solve(self, start=None, start_nodes: int = 1000):
         if self.model is not None and self.model.getNumberOfIntegerVariables() > 0:
-            self.branchAndCut()
+            self.branchAndCut(start, start_nodes)
         else:
             self.simplex()
         self.updateVariableValues()
