@@ -228,8 +228,7 @@ struct RoundExchange {
         scratch.assign((size_t)n * n_ranks, 0.0);
         memcpy(&scratch[(size_t)opts->rank * n], v, sizeof(double) * n);
         if (opts->all_gather(opts->user, scratch.data(), (int64_t)sizeof(double) * n)) return fail(JSLP_E_INVALID, "all_gather hook failed");
-        for (int r = 0; r < n_ranks; r++)
-            for (int k = 0; k < n; k++) v[k] = r == 0 ? scratch[k] : std::min(v[k], scratch[(size_t)r * n + k]);
+        jslp_bnb::fold_min(scratch.data(), n_ranks, n, v);
         return JSLP_OK;
     }
     int gather(void *buf, int64_t bytes_per_rank) {
@@ -491,7 +490,7 @@ static int branch_and_cut(jslp_tab *t, const jslp_bnb_opts *opts, const StartSet
         const bool sharded = n_ranks > 1 && iterations > 0 && !t->use_mir && (opts->shard_policy == 1 || !resident);
         std::vector<Branch *> mine;
         for (size_t i = 0; i < todo.size(); i++)
-            if (!sharded || (int)(i % n_ranks) == rank) mine.push_back(todo[i]);
+            if (!sharded || deal_rank(i, n_ranks) == rank) mine.push_back(todo[i]);
         if (resident) {
             if (!mine.empty()) {
                 int rc = eval_nodes_resident(t, mine.data(), (int)mine.size(), check_cycles);
@@ -510,14 +509,13 @@ static int branch_and_cut(jslp_tab *t, const jslp_bnb_opts *opts, const StartSet
         }
         count += (int64_t)mine.size();
         if (sharded) {  // all-gather the summaries: rank-major blocks of `per` records
-            const int per = (int)((todo.size() + n_ranks - 1) / n_ranks);
-            wire.assign((size_t)per * n_ranks * WIRE_DOUBLES, 0.0);
-            for (size_t j = 0; j < mine.size(); j++)
-                to_wire(mine[j]->ev, &wire[((size_t)rank * per + j) * WIRE_DOUBLES]);
-            int rc = ex.gather(wire.data(), (int64_t)per * WIRE_DOUBLES * 8);
-            if (rc) return rc;
+            const WireDeal deal(todo.size(), n_ranks);
+            wire.assign((size_t)deal.per * n_ranks * WIRE_DOUBLES, 0.0);
             for (size_t i = 0; i < todo.size(); i++)
-                from_wire(todo[i]->ev, &wire[((size_t)(i % n_ranks) * per + i / n_ranks) * WIRE_DOUBLES]);
+                if (deal_rank(i, n_ranks) == rank) to_wire(todo[i]->ev, &wire[deal.slot(i) * WIRE_DOUBLES]);
+            int rc = ex.gather(wire.data(), (int64_t)deal.per * WIRE_DOUBLES * 8);
+            if (rc) return rc;
+            for (size_t i = 0; i < todo.size(); i++) from_wire(todo[i]->ev, &wire[deal.slot(i) * WIRE_DOUBLES]);
         }
         return JSLP_OK;
     };

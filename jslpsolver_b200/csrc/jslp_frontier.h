@@ -7,6 +7,7 @@
 // ranks all-gather per node.
 #pragma once
 
+#include <algorithm>
 #include <cmath>
 #include <cstdint>
 #include <cstring>
@@ -251,6 +252,25 @@ struct Tree {
         return root ? SNAPSHOT : NEXT;
     }
 };
+
+// The deal of a sharded round (n_ranks > 1): node i of the round, in pop order, is evaluated by rank i % n_ranks.
+static inline int deal_rank(size_t i, int n_ranks) { return (int)(i % (size_t)n_ranks); }
+
+// Where a sharded round's results meet: a rank-major buffer of n_ranks blocks of `per` records, per = ceil(n / n_ranks)
+// for a round of n nodes.  Node i's record is the (i / n_ranks)-th of its rank's block; the last ranks' blocks end in
+// unused records when n is not a multiple of n_ranks, and a rank with no node of the round sends only those.
+struct WireDeal {
+    int n_ranks, per;
+    WireDeal(size_t n, int ranks) : n_ranks(ranks), per((int)((n + (size_t)ranks - 1) / (size_t)ranks)) {}
+    size_t slot(size_t i) const { return (size_t)deal_rank(i, n_ranks) * per + i / (size_t)n_ranks; }
+};
+
+// The element-wise min of a round's all-reduce when it is carried by an all-gather: blocks holds n_ranks rank-major
+// blocks of n doubles, v[k] becomes the smallest k-th entry over every rank's block.
+static inline void fold_min(const double *blocks, int n_ranks, int n, double *v) {
+    for (int r = 0; r < n_ranks; r++)
+        for (int k = 0; k < n; k++) v[k] = r == 0 ? blocks[k] : std::min(v[k], blocks[(size_t)r * n + k]);
+}
 
 static const int WIRE_DOUBLES = 16;  // all-gather record per node (128 bytes)
 static void to_wire(const NodeEval &e, double *w) {

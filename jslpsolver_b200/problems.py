@@ -358,6 +358,27 @@ def half_tie_mip_model(n_ints: int, group: int = 8, seed: int = 12345) -> dict:
             "constraints": constraints, "variables": variables, "ints": {f"x{i}": 1 for i in range(n_ints)}}
 
 
+def priority_tie_mip_model(n_objectives: int, n_items: int = 10, seed: int = 2) -> dict:
+    """A 0/1 MIP whose integral optima tie on the main objective and are told apart only by soft constraints: maximise
+    the number of items picked under one capacity row (weights U{2..5}, capacity half their sum plus one), so every
+    optimal plan picks the same number of items.  Soft constraint p = 1..n_objectives (`max: 0`, priority p, weight
+    U{1..3}) penalises picked items: priorities 1..n_objectives - 1 cover every item, so every optimal plan violates
+    them alike, and the last covers a random third of the items and decides between the optima.  Each distinct priority
+    is one optional objective (Tableau.optionalObjectives), so the model has exactly n_objectives of them, and the
+    branch-and-cut incumbent among tied plans is chosen by comparing them (branch-and-cut.ts:107-127)."""
+    rng = np.random.default_rng(seed)
+    w = rng.integers(2, 6, size=n_items)
+    variables = {f"x{j}": {"count": 1.0, "cap": float(w[j])} for j in range(n_items)}
+    constraints = {"cap": {"max": float(w.sum() // 2 + 1)}}
+    for p in range(1, n_objectives + 1):
+        items = range(n_items) if p < n_objectives else rng.choice(n_items, size=max(1, n_items // 3), replace=False)
+        for j in items:
+            variables[f"x{j}"][f"soft{p}"] = 1.0
+        constraints[f"soft{p}"] = {"max": 0.0, "priority": p, "weight": float(rng.integers(1, 4))}
+    return {"name": f"PriorityTieMIP_{n_objectives}_{n_items}_seed{seed}", "optimize": "count", "opType": "max",
+            "constraints": constraints, "variables": variables, "binaries": {f"x{j}": 1 for j in range(n_items)}}
+
+
 # ---- the reference's stress families (solver.stress.test.ts:41-215 solves them at 10..50 variables) ----------
 # Same shapes and distributions as problem-generator.ts's families, drawn from numpy's stream; every model is a
 # plain jsLPSolver JSON dict, so every implementation that is compared (and an outside solver) sees the same instance.
