@@ -461,8 +461,10 @@ static int branch_and_cut(jslp_tab *t, const jslp_bnb_opts *opts, const StartSet
         return JSLP_OK;
     };
 
-    // The tree's scalars are the tab's: node evaluations on the single-tableau path and keep_solutions' re-solves
-    // change the tab's between commits, and the commit reads them (Tableau.evaluation of an infeasible node's log row).
+    // The tab's scalars as the call finds them become the tree's (the root's log row reads Tableau.evaluation when the
+    // root is infeasible); from then on the tree's are the authority and store() copies them to the tab after every
+    // round and commit.  A node LP run in place on the single-tableau path sets the tab's evaluation when it runs, not
+    // when its turn to commit comes, and keep_solutions' re-solves set it again: neither may reach the tree.
     auto load = [&] {
         tree.feasible = t->feasible; tree.bounded = t->bounded; tree.evaluation = t->evaluation;
         tree.bestPossibleEval = t->bestPossibleEval; tree.simplexIters = t->simplexIters; tree.isIntegral = t->isIntegralFlag;
@@ -596,6 +598,7 @@ static int branch_and_cut(jslp_tab *t, const jslp_bnb_opts *opts, const StartSet
     double eval_ms = 0, commit_ms = 0, root_ms = 0, final_ms = 0;
     t->node_kernel_ns = 0;
     bool stop = false;
+    load();
     while (!stop && !branches.empty() && tree.toleranceFlag) {
         // ---- speculate: evaluate the next K un-evaluated open nodes in pop order ---------------
         const int width = iterations == 0 ? 1 : K;  // the root decides everything: alone
@@ -607,6 +610,7 @@ static int branch_and_cut(jslp_tab *t, const jslp_bnb_opts *opts, const StartSet
             rounds++;
             int rc = eval_round(todo, U, nodes);
             if (rc) return rc;
+            store();  // a speculated node's evaluation is the commit's to write
         }
         tree.put_back(taken);
         if (iterations == 0) root_ms += ms_since(t_eval);
@@ -626,7 +630,6 @@ static int branch_and_cut(jslp_tab *t, const jslp_bnb_opts *opts, const StartSet
 
         // ---- commit sequentially in the reference's exact order ---------------------------------
         for (;;) {
-            load();
             const Tree::Step st = tree.step(rule, [&] { return n_ranks > 1 ? round_time_up : time_up(); });
             store();
             if (st == Tree::DONE || st == Tree::ROUND) break;

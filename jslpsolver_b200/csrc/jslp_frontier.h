@@ -207,7 +207,9 @@ struct Tree {
         const NodeEval ev = active->ev;
         iterations++;
         feasible = ev.feasible; bounded = ev.bounded;
-        if (ev.feasible) evaluation = ev.evaluation;
+        // Tableau.evaluation is what the node's last optimal (or unbounded) solve set; an infeasible node keeps the
+        // previous value, except under useMIRCuts when a solve before the infeasible one was optimal
+        if (ev.feasible || ev.optimal) evaluation = ev.evaluation;
         if (ev.optimal) {  // setEvaluation + simplexIters (tableau.ts:420-430, simplex.ts:266-267)
             if (simplexIters == 0) bestPossibleEval = ev.n_optimal >= 0 ? ev.first_eval : ev.evaluation;
             simplexIters += ev.n_optimal >= 0 ? ev.n_optimal : 1;

@@ -79,7 +79,7 @@ def same(m, sol, simplified, ref):
     for i in range(len(ol)):
         a, b = gl[i], ol[i]
         assert all(a[k] == b[k] for k in (0, 1, 2, 4, 5, 7)) and bits(a[6]) == bits(b[6]), (i, a, b)
-        assert not b[2] or bits(a[3]) == bits(b[3]), (i, a, b)
+        assert bits(a[3]) == bits(b[3]), (i, a, b)
     st, fin = t.lastBnbStatus, res["o"].state()
     assert bits(st.evaluation) == bits(fin.evaluation)
     assert (st.feasible, st.bounded, st.iterations, bool(st.is_integral)) == \
