@@ -499,6 +499,9 @@ napi_value tab_branch_and_cut(napi_env env, napi_callback_info info) {
         napi_set_element(env, sols, (uint32_t)i, s);
     }
     napi_set_named_property(env, r, "solutions", sols);
+    set_num(env, r, "cycleRedosKernel", (double)st.cycle_redos_kernel);
+    set_num(env, r, "cycleRedosSlots", (double)st.cycle_redos_slots);
+    set_num(env, r, "cycleRedosPruned", (double)st.cycle_redos_pruned);
     return r;
 }
 

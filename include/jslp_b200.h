@@ -513,6 +513,12 @@ typedef struct {
     int64_t slot_pivots;   /* pivots executed in HBM node slots (jslp_slots.cuh), this rank             */
     double slot_ms;        /* wall time of the slot-batch graphs, this rank                              */
     double slot_bytes;     /* algorithmic bytes of those pivots: 16 * H_node * stride each               */
+    /* Node LPs whose pivot log repeated a block of (leaving, entering) pairs and that were solved again one after
+     * another on the single tableau, where the reference's stop-before-the-repeat rule is exact; this rank.  */
+    int64_t cycle_redos_kernel; /* cycles seen in the shared-memory node kernel's logs                       */
+    int64_t cycle_redos_slots;  /* cycles seen in the node slots' logs, re-solved                            */
+    int64_t cycle_redos_pruned; /* cycles seen in the node slots' logs, dropped unsolved: by the end of the
+                                   round an incumbent below the node's relaxed evaluation was known           */
 } jslp_bnb_status;
 
 int jslp_branch_and_cut(jslp_tab *root, const jslp_bnb_opts *opts, jslp_bnb_status *out,

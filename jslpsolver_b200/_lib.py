@@ -59,7 +59,8 @@ class BnbStatus(C.Structure):
         ("host_eval_ms", C.c_double), ("host_commit_ms", C.c_double),
         ("host_root_ms", C.c_double), ("host_final_ms", C.c_double), ("node_kernel_ms", C.c_double),
         ("timed_out", C.c_int32), ("n_solutions", C.c_int32), ("nodes_pruned", C.c_int64),
-        ("collectives", C.c_int64), ("slot_pivots", C.c_int64), ("slot_ms", C.c_double), ("slot_bytes", C.c_double)]
+        ("collectives", C.c_int64), ("slot_pivots", C.c_int64), ("slot_ms", C.c_double), ("slot_bytes", C.c_double),
+        ("cycle_redos_kernel", C.c_int64), ("cycle_redos_slots", C.c_int64), ("cycle_redos_pruned", C.c_int64)]
 
 
 class StartStatus(C.Structure):  # jslp_start_status

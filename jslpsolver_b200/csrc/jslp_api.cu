@@ -154,6 +154,7 @@ struct jslp_tab {
     std::vector<StoredSolution> solutions;  // keep_solutions (branch-and-cut.ts:143-153)
     int64_t slot_pivots = 0;
     double slot_ms = 0, slot_bytes = 0;
+    int64_t cycle_redos_kernel = 0, cycle_redos_slots = 0, cycle_redos_pruned = 0;  // jslp_bnb_status
     ResidentBufs rbufs;
     NodeSlots slots;        // K3: HBM-resident node batch (jslp_slots.cuh)
     int use_mir = 0;        // model.useMIRCuts (JSLP_OPT_USE_MIR_CUTS)

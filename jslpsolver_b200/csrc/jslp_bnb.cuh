@@ -343,7 +343,8 @@ static int eval_nodes_slots(jslp_tab *t, jslp_bnb::Branch *const *nodes, int n, 
         }
     }
     for (int i : redo) {
-        if (nodes[i]->relaxedEvaluation > *U) { (*pruned)++; continue; }
+        if (nodes[i]->relaxedEvaluation > *U) { (*pruned)++; t->cycle_redos_pruned++; continue; }
+        t->cycle_redos_slots++;
         rc = eval_node_streaming(t, *nodes[i], check_cycles, nodes[i]->ev);
         if (rc) return rc;
     }
@@ -383,6 +384,7 @@ static int eval_nodes_resident(jslp_tab *t, jslp_bnb::Branch *const *nodes, int 
     for (int i = 0; i < n; i++) {
         const NodeResult &r = rb.h_out[i].r;
         if (r.overflow || hit[i] >= 0) {
+            t->cycle_redos_kernel += hit[i] >= 0;
             redo.push_back(i);  // second pass: the HBM path may reuse rb's buffers
             continue;
         }
@@ -440,6 +442,7 @@ static int branch_and_cut(jslp_tab *t, const jslp_bnb_opts *opts, const StartSet
     t->saved.valid = false;
     t->isIntegralFlag = 0;
     t->slot_pivots = 0; t->slot_ms = 0; t->slot_bytes = 0;
+    t->cycle_redos_kernel = 0; t->cycle_redos_slots = 0; t->cycle_redos_pruned = 0;
     int K = opts->max_spec_batch > 0 ? opts->max_spec_batch : 16;  // any width commits in the same order
     std::vector<double> wire;
     RoundExchange ex{opts, n_ranks, {}, 0};
@@ -691,6 +694,8 @@ static int branch_and_cut(jslp_tab *t, const jslp_bnb_opts *opts, const StartSet
         out->timed_out = timed_out ? 1 : 0; out->n_solutions = (int)t->solutions.size();
         out->nodes_pruned = pruned; out->collectives = ex.collectives;
         out->slot_pivots = t->slot_pivots; out->slot_ms = t->slot_ms; out->slot_bytes = t->slot_bytes;
+        out->cycle_redos_kernel = t->cycle_redos_kernel; out->cycle_redos_slots = t->cycle_redos_slots;
+        out->cycle_redos_pruned = t->cycle_redos_pruned;
     }
     return JSLP_OK;
 }

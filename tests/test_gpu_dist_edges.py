@@ -32,7 +32,8 @@ pytestmark = pytest.mark.gpu
 
 WORKER = os.path.join(ROOT, "tests", "dist_edges_worker.py")
 WORK_COUNTERS = {"nodes_evaluated", "nodes_pruned", "gpu_ms", "kernel_launches", "host_eval_ms", "host_commit_ms",
-                 "host_root_ms", "host_final_ms", "node_kernel_ms", "slot_pivots", "slot_ms", "slot_bytes"}
+                 "host_root_ms", "host_final_ms", "node_kernel_ms", "slot_pivots", "slot_ms", "slot_bytes",
+                 "cycle_redos_kernel", "cycle_redos_slots", "cycle_redos_pruned"}
 OPT_NODE_SLOTS, OPT_NODE_LOG_CAP = 10, 14
 
 
