@@ -246,6 +246,24 @@ int jslp_scenario_batch(jslp_tab *tab, const jslp_scenario_edit *edits, const in
                         int check_cycles, int32_t *status, double *eval_raw, int32_t *p1, int32_t *p2, double *rhs,
                         int32_t *vrow);
 
+/* The recourse LPs of one iteration of a two-stage stochastic LP, DESIGN.md section 2u.  Scenario s is
+ * edits[offsets[s] .. offsets[s+1]) as jslp_scenario_batch runs it, with the cycle check on; status .. vrow are that
+ * call's outputs, bit for bit, and so is the state on return.  Beyond them, per scenario:
+ *   cert_rhs[s]  column 0 of the certificate row: row 0 when the scenario is optimal; when it is infeasible, the row
+ *                phase 1 stopped at (column 0 below -precision, no entering column: a Farkas row); NaN otherwise
+ *   alpha        n_first entries at s * n_first: alpha[j] = sum over i in increasing order of u[i] * tech[(ts * n_rows
+ *                + i) * n_first + j] (unfused), ts = s when tech_per_case, else 0.  u[i] is the certificate row's
+ *                multiplier of the row whose slack label is rows[i]: its entry when the label is non-basic, 1 or 0 when
+ *                it is basic in or off the row; all 0 without a certificate.  tech holds each row's coefficients of the
+ *                first-stage variables with the row's tableau sign (negated for a lower-bound row), so that column 0
+ *                of the certificate row moves by -alpha . dx when the first stage moves by dx.
+ * rows are distinct labels of the tableau, n_rows >= 0, n_first >= 0 (JSLP_E_INVALID otherwise).  No optional
+ * objectives (JSLP_E_UNSUPPORTED). */
+int jslp_recourse_batch(jslp_tab *tab, const jslp_scenario_edit *edits, const int32_t *offsets, int n_scenarios,
+                        const int32_t *rows, int n_rows, const double *tech, int n_first, int tech_per_case,
+                        int32_t *status, double *eval_raw, int32_t *p1, int32_t *p2, double *rhs, int32_t *vrow,
+                        double *cert_rhs, double *alpha);
+
 /* Warm-start crash, DESIGN.md section 2f: for each label enter[k] in order, pivot it into the basis on the row with the
  * largest |M[r,c]| among the rows r >= 1 whose basic label l has leave[l] != 0 and M[r,c] < -P || P < M[r,c] (lowest
  * row on ties); leave has one byte per label (n_index, see jslp_tab_info).  out[4k .. 4k+3] = (label, row, column,

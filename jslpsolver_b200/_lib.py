@@ -117,6 +117,7 @@ SYMBOLS = [
     ("jslp_parametric", C.c_int, [P, C.c_int, P, P, C.c_int, C.c_double, C.c_double, C.c_int, P, P, P, P,
                                   C.POINTER(C.c_int), C.POINTER(C.c_int), P, P]),
     ("jslp_scenario_batch", C.c_int, [P, P, P, C.c_int, C.c_int, P, P, P, P, P, P]),
+    ("jslp_recourse_batch", C.c_int, [P, P, P, C.c_int, P, C.c_int, P, C.c_int, C.c_int, P, P, P, P, P, P, P, P]),
     ("jslp_crash", C.c_int, [P, P, C.c_int, P, P, C.POINTER(C.c_int)]),
     ("jslp_frontier", C.c_int, [P, P, C.c_int, C.c_int, P, P, P, P, P, P, C.POINTER(C.c_int), C.POINTER(C.c_int), P, P,
                                 P, C.POINTER(C.c_int), P, P]),

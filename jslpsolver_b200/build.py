@@ -8,7 +8,7 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "csrc", "jslp_api.cu")
-DEPS = [SRC] + [os.path.join(HERE, "csrc", f) for f in ("jslp_kernels.cuh", "jslp_step.cuh", "jslp_node_kernel.cuh", "jslp_slots.cuh", "jslp_dynamic.cuh", "jslp_comm.cuh", "jslp_bnb_enhanced.cuh", "jslp_batch.cuh", "jslp_bnb.cuh", "jslp_sensitivity.cuh", "jslp_iis.cuh", "jslp_parametric.cuh", "jslp_scenario.cuh", "jslp_crash.cuh", "jslp_frontier.cuh", "jslp_face.cuh", "jslp_bound.cuh", "jslp_lex.cuh", "jslp_elastic.cuh", "jslp_cone.cuh", "jslp_pool.cuh", "jslp_conflict.cuh", "jslp_forest.cuh", "jslp_frontier.h", "jslp_cycles.h", "jslp_hostmath.h")] + [
+DEPS = [SRC] + [os.path.join(HERE, "csrc", f) for f in ("jslp_kernels.cuh", "jslp_step.cuh", "jslp_node_kernel.cuh", "jslp_slots.cuh", "jslp_dynamic.cuh", "jslp_comm.cuh", "jslp_bnb_enhanced.cuh", "jslp_batch.cuh", "jslp_bnb.cuh", "jslp_sensitivity.cuh", "jslp_iis.cuh", "jslp_parametric.cuh", "jslp_scenario.cuh", "jslp_recourse.cuh", "jslp_crash.cuh", "jslp_frontier.cuh", "jslp_face.cuh", "jslp_bound.cuh", "jslp_lex.cuh", "jslp_elastic.cuh", "jslp_cone.cuh", "jslp_pool.cuh", "jslp_conflict.cuh", "jslp_forest.cuh", "jslp_frontier.h", "jslp_cycles.h", "jslp_hostmath.h")] + [
     os.path.join(os.path.dirname(HERE), "include", "jslp_b200.h")]
 OUT = os.path.join(HERE, "libjslp_b200.so")
 

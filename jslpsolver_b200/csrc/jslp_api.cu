@@ -1364,6 +1364,7 @@ extern "C" int jslp_pivot_log(jslp_tab *t, int32_t *entries, int cap, int *n) {
 #include "jslp_iis.cuh"
 #include "jslp_parametric.cuh"
 #include "jslp_scenario.cuh"
+#include "jslp_recourse.cuh"
 #include "jslp_crash.cuh"
 #include "jslp_frontier.cuh"
 #include "jslp_face.cuh"

@@ -96,6 +96,13 @@ struct NodeBatchDev {
     const int *edit_off;
     double *out_rhs;
     int *out_vrow;
+    // scenario launches with cert_u set (jslp_recourse_batch): node n writes the multipliers of its certificate row
+    // (row 0 at an optimum, the row phase 1 stopped at when infeasible) to cert_u + n * cert_n, entry cert_pos[l] for
+    // every label l < cert_labels with cert_pos[l] >= 0: the row's entry when l is non-basic, its unit entry when l is
+    // basic; +0 throughout when there is no certificate (device memory).  Not read by the other modes.
+    double *cert_u;
+    const int *cert_pos;
+    int cert_n, cert_labels;
     int cost_edits;
     int n_inline;         // > 0: cut_off_inline holds the n_inline + 1 offsets (saves a PCIe round trip)
     int cut_off_inline[NODE_INLINE_OFF + 1];
@@ -552,6 +559,26 @@ __global__ void __launch_bounds__(NODE_THREADS) k_node_batch(const TabDev *Tp, c
     }
 
     if (tid == 0) tl3 = globaltimer_ns() - t_start;
+    if constexpr (SCENARIO)
+        if (nb.cert_u != nullptr) {
+            // the certificate row's multipliers of the requested rows, through the final labels (DESIGN.md 2u); sc.r
+            // is still the row whose phase-1 column scan found no entering column
+            const int st = s_fin[0], cr = st == ST_OPTIMAL ? 0 : st == ST_INFEASIBLE ? sc.r : -1;
+            double *u = nb.cert_u + (size_t)node * nb.cert_n;
+            if (cr < 0) {
+                for (int i = tid; i < nb.cert_n; i += NT) u[i] = 0.0;
+            } else {
+                const double *crow = Ms + (size_t)slot[cr] * Ws;
+                for (int c = 1 + tid; c < W; c += NT) {
+                    const int l = vcol[c], i = l >= 0 && l < nb.cert_labels ? nb.cert_pos[l] : -1;
+                    if (i >= 0) u[i] = crow[c];
+                }
+                for (int r = 1 + tid; r < Hn; r += NT) {
+                    const int l = vrow[r], i = l >= 0 && l < nb.cert_labels ? nb.cert_pos[l] : -1;
+                    if (i >= 0) u[i] = r == cr ? 1.0 : 0.0;
+                }
+            }
+        }
     // isIntegral / most fractional variable over the final RHS column
     for (int r = tid; r < Hn; r += NT) rhs[r] = Ms[(size_t)slot[r] * Ws];
     __syncthreads();

@@ -23,6 +23,56 @@ static bool resolve_edit(const HostMaps &m, const jslp_scenario_edit &e, EditDev
     return true;
 }
 
+// The certificate outputs of jslp_recourse_batch (DESIGN.md 2u): the multipliers of n_rows row labels per scenario,
+// to d_u + s * n_rows (device), at the position pos[label] (host; d_pos on the device) of each label.
+struct RecourseCert {
+    std::vector<int> pos;
+    const int *d_pos;
+    double *d_u;
+    int n_rows;
+};
+
+// The certificate row of a scenario that ended with `status` and final column 0 `rhs` (H entries): row 0 at an
+// optimum; when infeasible, the row phase 1 stopped at -- the first most negative entry below -precision, which is the
+// row its last selection took (simplex.ts:38-54) and which no pivot has touched since; -1 otherwise.
+static int cert_row(const jslp_tab *t, int status, const double *rhs) {
+    if (status == SCEN_OPTIMAL) return 0;
+    if (status != SCEN_INFEASIBLE) return -1;
+    int r0 = -1;
+    double v = -t->precision;
+    for (int r = 1; r < t->H; r++)
+        if (rhs[r] < v) { v = rhs[r]; r0 = r; }
+    return r0;
+}
+
+// The certificate multipliers of scenario s on the single-tableau path, whose final state is the current tableau: its
+// certificate row in one contiguous copy (the tableau is row-major), gathered through the final labels as
+// k_node_batch<NODE_SCENARIO> gathers them, to d_u + s * n_rows.
+static int cert_sequential(jslp_tab *t, const RecourseCert &c, int s, int status, const double *rhs,
+                           const int32_t *vrow) {
+    std::vector<double> u((size_t)c.n_rows, 0.0);
+    const int cr = cert_row(t, status, rhs);
+    cudaStream_t st = t->ctx->stream;
+    if (cr >= 0) {
+        std::vector<double> row((size_t)t->W);
+        std::vector<int> vcol((size_t)t->W);
+        CK(cudaMemcpyAsync(row.data(), t->hd.M + (size_t)cr * t->stride, sizeof(double) * (size_t)t->W,
+                           cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(vcol.data(), t->hd.vcol, sizeof(int) * (size_t)t->W, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        const int nl = (int)c.pos.size();
+        for (int k = 1; k < t->W; k++)
+            if (vcol[k] >= 0 && vcol[k] < nl && c.pos[vcol[k]] >= 0) u[c.pos[vcol[k]]] = row[k];
+        for (int r = 1; r < t->H; r++)
+            if (vrow[r] >= 0 && vrow[r] < nl && c.pos[vrow[r]] >= 0) u[c.pos[vrow[r]]] = r == cr ? 1.0 : 0.0;
+    }
+    if (c.n_rows > 0)
+        CK(cudaMemcpyAsync(c.d_u + (size_t)s * c.n_rows, u.data(), sizeof(double) * (size_t)c.n_rows,
+                           cudaMemcpyHostToDevice, st));
+    CK(cudaStreamSynchronize(st));
+    return JSLP_OK;
+}
+
 // One scenario on the single-tableau path, from the private snapshot.
 static int scenario_sequential(jslp_tab *t, const jslp_scenario_edit *e, int n, int check_cycles, int32_t *status,
                                double *eval_raw, int32_t *p1, int32_t *p2, double *rhs, int32_t *vrow) {
@@ -45,7 +95,7 @@ static int scenario_sequential(jslp_tab *t, const jslp_scenario_edit *e, int n, 
 // histories, as eval_nodes_resident) or that hit the pivot or log cap go to redo.
 static int scenario_resident(jslp_tab *t, const std::vector<EditDev> &res, const int32_t *offsets, int s0, int n,
                              int check_cycles, int32_t *status, double *eval_raw, int32_t *p1, int32_t *p2,
-                             double *rhs, int32_t *vrow, std::vector<int> &redo) {
+                             double *rhs, int32_t *vrow, const RecourseCert *cert, std::vector<int> &redo) {
     ResidentBufs &rb = t->rbufs;
     const int H0 = t->H;
     const Snapshot &src = t->snaps[2];
@@ -69,6 +119,12 @@ static int scenario_resident(jslp_tab *t, const std::vector<EditDev> &res, const
     nb.cut_off = (const int *)(base + b_off);
     nb.edits = (const EditDev *)(base + b_ed);
     nb.out_rhs = (double *)(base + b_rhs); nb.out_vrow = (int *)(base + b_vrow);
+    if (cert) {
+        nb.cert_u = cert->d_u + (size_t)s0 * cert->n_rows;
+        nb.cert_pos = cert->d_pos;
+        nb.cert_n = cert->n_rows;
+        nb.cert_labels = (int)cert->pos.size();
+    }
     if (n <= NODE_INLINE_OFF) {
         nb.n_inline = n;
         for (int i = 0; i <= n; i++) nb.cut_off_inline[i] = off[i];
@@ -89,24 +145,30 @@ static int scenario_resident(jslp_tab *t, const std::vector<EditDev> &res, const
     return JSLP_OK;
 }
 
-extern "C" int jslp_scenario_batch(jslp_tab *t, const jslp_scenario_edit *edits, const int32_t *offsets, int n_scenarios,
-                                   int check_cycles, int32_t *status, double *eval_raw, int32_t *p1, int32_t *p2,
-                                   double *rhs, int32_t *vrow) {
+// The argument checks of jslp_scenario_batch and jslp_recourse_batch (`what` names the caller in the messages).
+static int scenario_check(jslp_tab *t, const jslp_scenario_edit *edits, const int32_t *offsets, int n_scenarios,
+                          int32_t *status, double *eval_raw, int32_t *p1, int32_t *p2, double *rhs, int32_t *vrow,
+                          const char *what) {
     if (!t) return fail(JSLP_E_INVALID, "tab is NULL");
+    const std::string w(what);
     if (n_scenarios < 0 || (n_scenarios > 0 && (!offsets || !status || !eval_raw || !p1 || !p2 || !rhs || !vrow)))
-        return fail(JSLP_E_INVALID, "scenario_batch: bad offsets / output arguments");
-    if (t->nOpt > 0) return fail(JSLP_E_UNSUPPORTED, "scenario_batch: optional objectives are not supported");
+        return fail(JSLP_E_INVALID, w + ": bad offsets / output arguments");
+    if (t->nOpt > 0) return fail(JSLP_E_UNSUPPORTED, w + ": optional objectives are not supported");
     if (n_scenarios == 0) return JSLP_OK;
-    int rc = batch_check_offsets({offsets}, n_scenarios, "scenario_batch");
+    int rc = batch_check_offsets({offsets}, n_scenarios, w);
     if (rc) return rc;
+    if (offsets[n_scenarios] > 0 && !edits) return fail(JSLP_E_INVALID, w + ": edits is NULL");
+    return JSLP_OK;
+}
+
+// jslp_scenario_batch once the arguments are checked (n_scenarios > 0) and the labels loaded into m; with cert set,
+// every scenario's certificate multipliers go to cert->d_u as well.
+static int scenario_run(jslp_tab *t, const HostMaps &m, const jslp_scenario_edit *edits, const int32_t *offsets,
+                        int n_scenarios, int check_cycles, int32_t *status, double *eval_raw, int32_t *p1, int32_t *p2,
+                        double *rhs, int32_t *vrow, const RecourseCert *cert) {
     const int n_edits = offsets[n_scenarios];
-    if (n_edits > 0 && !edits) return fail(JSLP_E_INVALID, "scenario_batch: edits is NULL");
-    CK(cudaSetDevice(t->ctx->device));
     // updateRightHandSide / updateCost resolved once against the labels: no edit pivots, so the positions are the
     // same for every scenario and every edit of it
-    HostMaps m;
-    rc = load_maps(t, m);
-    if (rc) return rc;
     std::vector<EditDev> res((size_t)n_edits);
     for (int i = 0; i < n_scenarios; i++)
         for (int k = offsets[i]; k < offsets[i + 1]; k++) {
@@ -117,7 +179,7 @@ extern "C" int jslp_scenario_batch(jslp_tab *t, const jslp_scenario_edit *edits,
             if (!resolve_edit(m, e, &res[k])) return fail(JSLP_E_INVALID, "scenario_batch: unknown constraint or variable index");
         }
     const CallerState caller(t);
-    rc = ensure_snapshot(t, 2);
+    int rc = ensure_snapshot(t, 2);
     if (rc) return rc;
     rc = snapshot_copy(t, 2, true);
     if (rc) return rc;
@@ -127,11 +189,14 @@ extern "C" int jslp_scenario_batch(jslp_tab *t, const jslp_scenario_edit *edits,
         t, n_scenarios, [&](int) { return H; }, true,
         [&](const int *idx, int m, std::vector<int> &redo) {
             return scenario_resident(t, res, offsets, idx[0], m, check_cycles, status, eval_raw, p1, p2, rhs, vrow,
-                                     redo);
+                                     cert, redo);
         },
         [&](int i) {
-            return scenario_sequential(t, edits + offsets[i], offsets[i + 1] - offsets[i], check_cycles, status + i,
-                                       eval_raw + i, p1 + i, p2 + i, rhs + (size_t)i * H, vrow + (size_t)i * H);
+            const int rc1 = scenario_sequential(t, edits + offsets[i], offsets[i + 1] - offsets[i], check_cycles,
+                                                status + i, eval_raw + i, p1 + i, p2 + i, rhs + (size_t)i * H,
+                                                vrow + (size_t)i * H);
+            if (rc1 || !cert) return rc1;
+            return cert_sequential(t, *cert, i, status[i], rhs + (size_t)i * H, vrow + (size_t)i * H);
         });
     // the caller's tableau, labels, staged pivot and record exactly as they were
     const int rc2 = snapshot_copy(t, 2, false);
@@ -139,4 +204,16 @@ extern "C" int jslp_scenario_batch(jslp_tab *t, const jslp_scenario_edit *edits,
     CK(cudaStreamSynchronize(t->ctx->stream));
     caller.restore(t);
     return rc;
+}
+
+extern "C" int jslp_scenario_batch(jslp_tab *t, const jslp_scenario_edit *edits, const int32_t *offsets, int n_scenarios,
+                                   int check_cycles, int32_t *status, double *eval_raw, int32_t *p1, int32_t *p2,
+                                   double *rhs, int32_t *vrow) {
+    int rc = scenario_check(t, edits, offsets, n_scenarios, status, eval_raw, p1, p2, rhs, vrow, "scenario_batch");
+    if (rc || n_scenarios == 0) return rc;
+    CK(cudaSetDevice(t->ctx->device));
+    HostMaps m;
+    rc = load_maps(t, m);
+    if (rc) return rc;
+    return scenario_run(t, m, edits, offsets, n_scenarios, check_cycles, status, eval_raw, p1, p2, rhs, vrow, nullptr);
 }

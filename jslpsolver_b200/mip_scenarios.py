@@ -24,22 +24,23 @@ from .tableau import solution_set
 WHAT = "Scenarios()"
 
 
-def _refuse(model: dict) -> None:
+def _refuse(model: dict, what: str = WHAT) -> None:
+    """The model options Scenarios() (and TwoStage(), as `what`) refuse."""
     opt = model.get("optimize")
     if isinstance(opt, dict) and len(object_keys(opt)) > 1:
-        raise ValueError(f"{WHAT} takes one objective: `optimize` has {len(object_keys(opt))}")
+        raise ValueError(f"{what} takes one objective: `optimize` has {len(object_keys(opt))}")
     if model.get("external"):
-        raise ValueError(f"{WHAT} does not support external solvers")
+        raise ValueError(f"{what} does not support external solvers")
     for spec in (model.get("constraints") or {}).values():
         if isinstance(spec, dict) and (spec.get("weight") is not None or spec.get("priority") is not None):
-            raise ValueError(f"{WHAT} does not support soft constraints (weight / priority)")
+            raise ValueError(f"{what} does not support soft constraints (weight / priority)")
     options = model.get("options") or {}
     if _truthy(model.get("timeout")) or (_truthy(options) and _truthy(options.get("timeout"))):
-        raise ValueError(f"{WHAT} does not support timeout: a wall-clock stop cannot be reproduced when trees share "
+        raise ValueError(f"{what} does not support timeout: a wall-clock stop cannot be reproduced when trees share "
                          "rounds")
     for key in ("useMIRCuts", "keep_solutions", "nodeSelection", "branching", "useIncremental"):
         if _truthy(options) and _truthy(options.get(key)):
-            raise ValueError(f"{WHAT} runs the default branch-and-cut service: options.{key} is not supported")
+            raise ValueError(f"{what} runs the default branch-and-cut service: options.{key} is not supported")
 
 
 def _one_objective(model: dict) -> dict:

@@ -17,6 +17,7 @@ from .polyopt import Polyopt
 from .pool import Pool as _pool
 from .repair import Repair as _repair
 from .repair_mip import RepairMIP as _repair_mip
+from .two_stage import TwoStage as _two_stage
 
 
 class Solver:
@@ -155,6 +156,15 @@ class Solver:
         only."""
         return _scenarios(self, model, cases, width, precision, validate)
 
+    def TwoStage(self, model: dict, cases, first, probabilities=None, *, gap=1e-9, absolute_gap=None,
+                 max_iterations=200, precision: Optional[float] = None, validate: bool = False) -> dict:
+        """A two-stage stochastic LP: the first-stage plan over the variables `first` that minimises (or maximises)
+        its cost plus the expected cost of each case's recourse plan, by the L-shaped method with every case's recourse
+        LP batched on the device (two_stage.py, DESIGN.md section 2u).  Cases take "rhs" and "cost" of second-stage
+        rows and variables as Scenarios() does, and "coefficients": {constraint: {first-stage variable: value}}."""
+        return _two_stage(self, model, cases, first, probabilities, gap=gap, absolute_gap=absolute_gap,
+                          max_iterations=max_iterations, precision=precision, validate=validate)
+
     def _instance(self, model: Any, precision: Optional[float]) -> Model:
         if isinstance(model, dict):
             options = model.get("options") or {}
@@ -249,6 +259,12 @@ def Conflict(model: dict, max_nodes=10000, width=None, depth=None, precision: Op
 
 def Scenarios(model: dict, cases, *, width=None, precision: Optional[float] = None, validate: bool = False) -> list:
     return solver.Scenarios(model, cases, width=width, precision=precision, validate=validate)
+
+
+def TwoStage(model: dict, cases, first, probabilities=None, *, gap=1e-9, absolute_gap=None, max_iterations=200,
+             precision: Optional[float] = None, validate: bool = False) -> dict:
+    return solver.TwoStage(model, cases, first, probabilities, gap=gap, absolute_gap=absolute_gap,
+                           max_iterations=max_iterations, precision=precision, validate=validate)
 
 
 def Variability(model: dict, gap=0.0, absolute_gap=0.0, variables=None, constraints=None, points=False,

@@ -776,6 +776,31 @@ class GpuTableau:
             p2.ctypes.data, rhs.ctypes.data, vrow.ctypes.data))
         return {"status": status, "eval_raw": eval_raw, "p1": p1, "p2": p2, "rhs": rhs, "vrow": vrow}
 
+    def recourse_batch(self, edits, offsets, rows, tech) -> dict:
+        """jslp_recourse_batch: scenario_batch's run of edits / offsets (cycle check on) and outputs, plus each
+        scenario's certificate: "cert_rhs" (column 0 of row 0 at an optimum, of the row phase 1 stopped at when
+        infeasible, NaN otherwise) and "alpha" (n x n_first), the certificate row's multipliers of the row labels `rows`
+        summed against `tech` -- one matrix (len(rows) x n_first) for every scenario, or one per scenario (n x len(rows)
+        x n_first) -- in the rows' tableau sign (DESIGN.md section 2u).  The tableau is unchanged."""
+        n, H = len(offsets) - 1, self.height
+        arr = self._edit_array([(edits, ())])
+        off = np.ascontiguousarray(offsets, dtype=np.int32)
+        lab = np.ascontiguousarray(rows, dtype=np.int32)
+        tec = np.ascontiguousarray(tech, dtype=np.float64)
+        per_case = int(tec.ndim == 3)
+        n_first = tec.shape[-1]
+        status, p1, p2 = (np.empty(n, dtype=np.int32) for _ in range(3))
+        eval_raw, cert_rhs = np.empty(n, dtype=np.float64), np.empty(n, dtype=np.float64)
+        rhs, vrow = np.empty((n, H), dtype=np.float64), np.empty((n, H), dtype=np.int32)
+        alpha = np.empty((n, n_first), dtype=np.float64)
+        _lib.check(self.context.lib.jslp_recourse_batch(
+            self._h(), arr, off.ctypes.data, n, lab.ctypes.data if len(lab) else None, len(lab),
+            tec.ctypes.data if tec.size else None, n_first, per_case, status.ctypes.data, eval_raw.ctypes.data,
+            p1.ctypes.data, p2.ctypes.data, rhs.ctypes.data, vrow.ctypes.data, cert_rhs.ctypes.data,
+            alpha.ctypes.data if alpha.size else None))
+        return {"status": status, "eval_raw": eval_raw, "p1": p1, "p2": p2, "rhs": rhs, "vrow": vrow,
+                "cert_rhs": cert_rhs, "alpha": alpha}
+
     def _adopt(self, h) -> "GpuTableau":
         """A GpuTableau over the tab handle h that the library derived from this one (face, bound, lex_next, elastic,
         cone): this tableau's precision, context, model, integer count, engine and options, no optional objectives,
